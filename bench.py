@@ -1,15 +1,16 @@
 #!/usr/bin/env python
-"""bench.py — octree insertion throughput (and render rate) on N B200s.
+"""bench.py — octree insertion throughput (and render rate) on N H100s.
 
-    python bench.py --gpus N --steps K --warmup W            # our sm_100a path
+    python bench.py --gpus N --steps K --warmup W            # our sm_90a path
     python bench.py --impl reference --gpus N --steps K ...  # the reference algorithm on host cores (oracle port)
+    python bench.py ... --dump-outputs DIR                   # also write the octree of the last timed step to DIR/*.npy
 
-A step is one pass of the hot path over one batch: 1 000 000 synthetic XYZRGBA points (16 B each) inserted into the
-growing octree by kernel_construct. The workload does NOT depend on --steps: at N = 1 it is BASELINE.json configs[2],
-the 350 M-point stream (Morro-Bay stand-in terrain, no dataset on the box), inserted from a freshly reset octree in
-350 spatially coherent 1 M-point batches; a timed PASS is the whole stream, the reported time is the median of
->= 5 passes from reset (SURVEY.md §8d), and ms_per_step is that time per 1 M-point batch. --steps only echoes into the
-line (and bounds the reference arm's CPU sample), --warmup batches are inserted untimed first.
+A step is one pass of the hot path over the whole stream: at N = 1 that is BASELINE.json configs[2], the 350 M-point
+stream (Morro-Bay stand-in terrain, generated on the device), inserted by kernel_construct from a freshly reset octree
+in 350 spatially coherent batches of 1 000 000 synthetic XYZRGBA points (16 B each). --warmup W untimed steps are run
+first, then --steps K timed steps; the reported time is the median of the K (SURVEY.md §8d), ms_per_step is that
+median and config.ms_per_batch the same time per 1 M-point batch. In the reference arm a step is one 1 M-point batch.
+The inputs depend only on --gpus and --batches, so runs with the same arguments insert identical points.
 
 With N > 1 every rank owns a complete builder and inserts its own 350 M-point scan tile of the same extent and density
 (tile g of a survey of N tiles): per-GPU work is identical to N = 1, scaling is weak, and there is no data-path
@@ -25,9 +26,9 @@ Numbers:
   e2e          same metric through the public API from pinned HOST memory: per step one 16 MB host->device copy
                and one 112-byte Stats read-back per launch inside the timed region
   roofline     kernel_construct: algorithmic bytes (16 in + 16 out + 32*s + 16*v per point, SURVEY.md §8d)
-               / summed launch time (CUDA events on the launch stream) against the measured HBM copy peak
-  reference_gpu  the UNMODIFIED reference kernels (oracle/_ref/*.cubin, compiled from /root/reference by
-               oracle/build_ref.cpp) through simlod_use_module on the same GPU, same buffers, same input, with their
+               / summed launch time (CUDA events on the launch stream) against the HBM peak (data sheet unless measured)
+  reference_gpu  the UNMODIFIED reference kernels (oracle/_ref/*.cubin, compiled from the original SimLOD sources
+               ($SIMLOD_REFERENCE) by oracle/build_ref.cpp) through simlod_use_module on the same GPU, same buffers, same input, with their
                native grids (1 block/SM construct, occupancy render): the numbers to beat (SURVEY.md §8d-i)
   render       kernel_render on the built octree, 6 cameras x {atomicMin, HQS}, with the per-frame HBM roofline
                (16 B/sample + 12*W*H, HQS 32 B/sample + 28*W*H) and the reference kernel beside it
@@ -62,12 +63,12 @@ def parse():
     ap.add_argument("--steps", type=int, default=20)
     ap.add_argument("--warmup", type=int, default=5)
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
-    ap.add_argument("--passes", type=int, default=5, help="timed passes over the whole stream (median reported)")
     ap.add_argument("--batches", type=int, default=CONFIG3_BATCHES, help="developer knob: batches of the stream (350 = config 3)")
     ap.add_argument("--cpu-sample-batches", type=int, default=16, help="batches of the stream the 1-thread CPU oracle inserts for cpu_baseline (about 6-10 s)")
     ap.add_argument("--no-render", action="store_true")
     ap.add_argument("--no-reference-gpu", action="store_true")
     ap.add_argument("--no-extras", action="store_true", help="skip the LAS / file-streamer / config-4 legs")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write the octree the last timed step built on rank 0 (canonical form and a seeded point sample) to DIR/*.npy")
     return ap.parse_args()
 
 
@@ -76,7 +77,7 @@ def workload_name(batches):
         batches, batches, batches)
 
 
-# ---- clocks sampled DURING the timed regions (B200_PROFILING.md) --------------------------------
+# ---- clocks sampled DURING the timed regions --------------------------------
 class ClockSampler:
     Q = "clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap"
 
@@ -134,19 +135,44 @@ def peaks():
             return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs, copy kernel)"
         except Exception:
             pass
-    return 6650.0, "fallback (B200_PROFILING.md, 6.65 TB/s)"
+    return 3350.0, "data sheet (NVIDIA H100 SXM, 3.35 TB/s HBM3)"
 
 
-def recorded_traffic(batches):
-    """DRAM bytes per kernel_construct launch of THIS workload from the committed ncu launch list, if one exists
-    (profiles/r02/ncu_construct_traffic_<batches>M.json, written by tools/ncu_traffic.py)."""
-    p = os.path.join(ROOT, "profiles", "r02", "ncu_construct_traffic_%dM.json" % batches)
-    if os.path.exists(p):
-        try:
-            return json.load(open(p))
-        except Exception:
-            return None
-    return None
+def dump_outputs(sim, out_dir):
+    """The octree in the device buffers, as the canonical form the tests compare (oracle.compare_canon): per node its
+    key, counters and chunk counts (octree_nodes.npy, columns = NODE_COLUMNS) and the hashes of its sorted point and
+    voxel-position multisets as 32-bit halves (octree_hashes.npy), plus the deterministic Stats fields (stats.npy).
+    Everything is an integer below 2^53, so float64 holds it exactly. So that a mismatch can be located, also a fixed,
+    seeded sample of the stored points: up to SAMPLE_POINTS of the sorted points of each of up to SAMPLE_LEAVES
+    non-empty leaves (sample_xyz.npy float32, sample_color.npy and sample_node.npy, the canonical node index, float64)."""
+    import oracle
+    os.makedirs(out_dir, exist_ok=True)
+    canon = oracle.canon_from_image(*sim.download_octree())
+    rec = canon.records
+    nodes = np.stack([rec[f].astype(np.float64) for f in NODE_COLUMNS], axis=1)
+    halves = [(rec[f] >> np.uint64(32)).astype(np.float64) for f in ("hashPoints", "hashVoxelPos")] + \
+             [(rec[f] & np.uint64(0xFFFFFFFF)).astype(np.float64) for f in ("hashPoints", "hashVoxelPos")]
+    st = sim.stats()
+    np.save(os.path.join(out_dir, "octree_nodes.npy"), nodes)
+    np.save(os.path.join(out_dir, "octree_hashes.npy"), np.stack(halves, axis=1))
+    np.save(os.path.join(out_dir, "stats.npy"), np.array([float(getattr(st, f)) for f in oracle.STATS_FIELDS]))
+    rng = np.random.default_rng(0)
+    leaves = np.nonzero((rec["isLeaf"] == 1) & (rec["numPoints"] > 0))[0]
+    picked = np.sort(rng.choice(leaves, min(SAMPLE_LEAVES, len(leaves)), replace=False))
+    xyz, color, node = [], [], []
+    for k in picked:
+        pts = canon.samples(int(k))
+        pts = pts[np.sort(rng.choice(len(pts), min(SAMPLE_POINTS, len(pts)), replace=False))]
+        xyz.append(np.stack([pts["x"], pts["y"], pts["z"]], axis=1))
+        color.append(pts["color"].astype(np.float64))
+        node.append(np.full(len(pts), float(k)))
+    np.save(os.path.join(out_dir, "sample_xyz.npy"), np.concatenate(xyz) if xyz else np.zeros((0, 3), np.float32))
+    np.save(os.path.join(out_dir, "sample_color.npy"), np.concatenate(color) if color else np.zeros(0))
+    np.save(os.path.join(out_dir, "sample_node.npy"), np.concatenate(node) if node else np.zeros(0))
+
+
+SAMPLE_LEAVES, SAMPLE_POINTS = 64, 1024
+NODE_COLUMNS = ("level", "X", "Y", "Z", "counter", "numPoints", "numVoxels", "numVoxelsStored", "isLeaf", "chunksPoints", "chunksVoxels")
 
 
 def cameras(box_max):
@@ -210,7 +236,7 @@ def bench_reference_gpu(device, dptr, n_batches, box, peak, ours_octree_sim):
     rasteriser was timed on (ref_render.cubin swapped in, its occupancy grid)."""
     import oracle
     from simlod_b200 import SimLOD
-    out = {"kernels": "oracle/_ref/ref_{construct,render,reset}.cubin = the unmodified /root/reference sources, NVRTC + nvJitLink as CudaModularProgram.h:84-98,214-239, sm_100"}
+    out = {"kernels": "oracle/_ref/ref_{construct,render,reset}.cubin = the unmodified original SimLOD sources ($SIMLOD_REFERENCE), NVRTC + nvJitLink as CudaModularProgram.h:84-98,214-239, sm_90"}
     if not all(os.path.exists(p) for p in oracle.REF_CUBINS.values()):
         out["unavailable"] = "oracle/_ref/*.cubin not built"
         return out
@@ -319,7 +345,7 @@ def bench_las(sim_device, host_batches, mn, mx):
                     best = (dt_t, threads)
             dt, threads = best
             out["cpu_baseline"] = {"value": round(n / dt / 1e6, 1), "unit": "Mpoints/s", "cores": threads, "kind": "reference",
-                                   "sample": "loadLasNative (LasLoader.cpp compiled from /root/reference) on %d M points from tmpfs in 250k-point batches, long-lived loader threads; best of 1 / 8 / all cores" % (n // 1000000)}
+                                   "sample": "loadLasNative (LasLoader.cpp compiled from the original SimLOD sources) on %d M points from tmpfs in 250k-point batches, long-lived loader threads; best of 1 / 8 / all cores" % (n // 1000000)}
         finally:
             if os.path.exists(path):
                 os.remove(path)
@@ -328,7 +354,7 @@ def bench_las(sim_device, host_batches, mn, mx):
 
 def bench_stream_file(sim_device, host_batches, mn, mx):
     """.simlod file (tmpfs, and cold from disk when the box has one) -> loader threads -> pinned pool -> ring -> octree, with
-    the reference's own loadFileNative (SimlodLoader.cpp compiled from /root/reference) timed beside it on the host cores."""
+    the reference's own loadFileNative (SimlodLoader.cpp compiled from the original SimLOD sources) timed beside it on the host cores."""
     import tempfile
     import oracle
     from simlod_b200 import SimLOD, data
@@ -361,7 +387,7 @@ def bench_stream_file(sim_device, host_batches, mn, mx):
                 if best is None or dt_t < best[0]:
                     best = (dt_t, threads)
             out["cpu_baseline"] = {"value": round(n / best[0] / 1e6, 1), "unit": "Mpoints/s", "cores": best[1], "kind": "reference",
-                                   "sample": "loadFileNative (SimlodLoader.cpp compiled from /root/reference), %d x 1M-point reads from tmpfs into host memory; best of 1 / 8 / all cores" % nb}
+                                   "sample": "loadFileNative (SimlodLoader.cpp compiled from the original SimLOD sources), %d x 1M-point reads from tmpfs into host memory; best of 1 / 8 / all cores" % nb}
         # cold file: the same scan on a disk-backed file system, its pages evicted before every run, read unbuffered (O_DIRECT)
         cold_path = os.path.join(tempfile.gettempdir(), "simlod_bench_cold_%d.simlod" % os.getpid())
         try:
@@ -555,9 +581,8 @@ def main():
             dist.barrier()
         torch.cuda.synchronize()
 
-    W, K = max(args.warmup, 0), args.steps
+    W, K = max(args.warmup, 0), max(args.steps, 1)
     NB = args.batches
-    passes = max(args.passes, 1)
     npts = NB * BATCH
     mn, mx = (0.0, 0.0, 0.0), data.TERRAIN_EXTENT
     peak, peak_src = peaks()
@@ -578,17 +603,17 @@ def main():
         sim._check(sim._lib.simlod_memcpy_dtoh(sim._ctx, host_ptr, dptr, npts * 16))
         t_gen = time.time() - t_gen
 
-        # warm-up: W batches (code, clocks, allocator paths), then start over
-        sim.reset()
-        if W:
-            sim.insert_device(dptr, min(W, NB) * BATCH)
+        # warm-up: W untimed steps (code, clocks, allocator paths)
+        timed_passes(sim, lambda: sim.insert_device(dptr, npts), npts, W, barrier, [])
         info0 = sim.launch_info()
 
-        # ---- timed region 1: inputs resident in HBM, median of `passes` passes over the whole stream ----------
-        ks, ts = timed_passes(sim, lambda: sim.insert_device(dptr, npts), npts, passes, barrier, windows)
+        # ---- timed region 1: inputs resident in HBM, median of K steps, each the whole stream from reset ----------
+        ks, ts = timed_passes(sim, lambda: sim.insert_device(dptr, npts), npts, K, barrier, windows)
         st = sim.stats()
         info1 = sim.launch_info()
-        launches_per_pass = (info1["launches"] - info0["launches"]) // passes - 2     # minus the reset kernel and the L2 flush fill
+        launches_per_pass = (info1["launches"] - info0["launches"]) // K - 2     # minus the reset kernel and the L2 flush fill
+        if args.dump_outputs and rank == 0:        # every rank builds its own tile; rank 0's is the N = 1 workload
+            dump_outputs(sim, args.dump_outputs)
         b = sim.buffers()
         ctl = sim.memcpy_dtoh(b.momentary + 80, 16).view(np.uint64)    # Ctl::spilledTotal, voxelsTotal (construct.cu)
         spilled_total, voxels_total = int(ctl[0]), int(ctl[1])
@@ -616,7 +641,7 @@ def main():
 
         # ---- timed region 2: end to end from pinned host memory (median of 3 passes) ----------------------
         info2 = sim.launch_info()
-        e_passes = min(3, passes)
+        e_passes = min(3, K)
         eks, ets = [], []
         e_wall = []
         for _ in range(e_passes):
@@ -665,14 +690,14 @@ def main():
                 for k, bidx in enumerate(sdist.shard_batches(total4, rank, world)):
                     sim.generate(sim.GEN_SHELL, d4 + k * BATCH * 16, total4 * BATCH, bidx * BATCH, BATCH, SHELL_SEED)
                 sim.set_box((0.0, 0.0, 0.0), (data.SHELL_CUBE,) * 3)
-                ks4, ts4 = timed_passes(sim, lambda: sim.insert_device(d4, nb4 * BATCH), nb4 * BATCH, min(3, passes), barrier, windows)
+                ks4, ts4 = timed_passes(sim, lambda: sim.insert_device(d4, nb4 * BATCH), nb4 * BATCH, min(3, K), barrier, windows)
                 st4 = sim.stats()
                 t4 = sdist.max_over_ranks(float(np.median(ts4)), dev)
                 tk4 = sdist.max_over_ranks(float(np.median(ks4)), dev)
                 tot4 = sdist.reduce_stats(st4, dev)
                 config4 = {"workload": "sphere shell R=1800 in a 4096^3 cube, %d M points in lat/lon tile order, rank g inserts the 1M-point batches b = g (mod %d): %d M points per GPU" % (total4, world, nb4),
                            "value": round(world * nb4 * BATCH / t4 / 1e3, 2), "unit": "Mpoints/s", "kernel_only": round(world * nb4 * BATCH / tk4 / 1e3, 2),
-                           "passes": min(3, passes), "octree": {k: tot4[k] for k in ("numNodes", "numPoints", "numVoxels")},
+                           "passes": min(3, K), "octree": {k: tot4[k] for k in ("numNodes", "numPoints", "numVoxels")},
                            "note": "per-GPU work changes with N here: a G-times sparser sample of a G-times denser shell has more nodes and voxels per point (DESIGN.md §8); `value` above keeps per-GPU work fixed instead"}
                 sim.device_free(d4)
                 sim.set_box(mn, mx)
@@ -713,26 +738,23 @@ def main():
         v_frac = voxels_total / npts
         alg_bytes = (32.0 + 32.0 * s_frac + 16.0 * v_frac) * npts          # this rank, one pass
         achieved = alg_bytes / (kernel_ms * 1e-3) / 1e9
-        traffic = recorded_traffic(NB)
         n_launch = max(launches_per_pass, 1)
         line = {
             "metric": METRIC, "value": round(value, 2), "unit": "Mpoints/s", "n_gpus": world, "steps": K, "warmup": W,
-            "ms_per_step": round(t_value / NB, 5), "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
+            "ms_per_step": round(t_value, 4), "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
             "dtype": "u32+f32", "data": "synthetic",
             "config": {"workload": workload_name(NB),
-                       "batch_points": BATCH, "points_per_gpu": npts, "steps_per_pass": NB, "timed_passes": passes,
-                       "timing": "median of %d passes, each the whole stream from reset (a step = one 1M-point batch; --steps does not size the workload); max over ranks of the per-rank median" % passes,
+                       "batch_points": BATCH, "points_per_gpu": npts, "batches_per_step": NB, "ms_per_batch": round(t_value / NB, 5),
+                       "timing": "median of %d steps, each the whole stream from reset, after %d untimed steps; max over ranks of the per-rank median" % (K, W),
                        "parallelism": "batch-sharded x%d (one %d-batch scan tile per GPU, no data-path collective)" % (world, NB),
-                       "l2": "inputs %d MB > L2 (126 MB); L2 flushed before each timed pass" % (npts * 16 // 1000000),
+                       "l2": "inputs %d MB > L2 (50 MB); L2 flushed before each timed pass" % (npts * 16 // 1000000),
                        "kernel_only_mpoints_per_s": round(all_pts / t_kernel / 1e3, 2),
-                       "pass_ms": [round(x, 3) for x in ts], "pass_kernel_ms": [round(x, 3) for x in ks],
+                       "step_ms": [round(x, 3) for x in ts], "step_kernel_ms": [round(x, 3) for x in ks],
                        "octree": {k: totals[k] for k in ("numNodes", "numInner", "numLeaves", "numPoints", "numVoxels", "allocatedBytes_persistent")},
                        "construct_blocks": info1["construct_blocks"], "datagen_s": round(t_gen, 1),
                        "data_generator": "simlod_generate (csrc/gen.cu), bit-identical to simlod_b200/data.py:terrain (tests/test_generators.py)"},
             "roofline": {"bound": "hbm", "kernel": "kernel_construct", "achieved": round(achieved, 2), "peak": peak, "unit": "GB/s",
                          "frac": round(achieved / peak, 5),
-                         "traffic": traffic.get("dram_bytes_per_launch") if traffic else None,
-                         "traffic_source": traffic.get("source") if traffic else None,
                          "peak_source": peak_src,
                          "algorithmic_bytes_per_point": round(alg_bytes / npts, 3), "spilled_fraction_s": round(s_frac, 4),
                          "voxels_per_point_v": round(v_frac, 4), "launches": launches_per_pass,
@@ -741,7 +763,7 @@ def main():
             "e2e": {"value": round(all_pts / t_e2e / 1e3, 2), "unit": "Mpoints/s", "h2d_bytes_per_step": BATCH * 16,
                     "d2h_bytes_per_step": round(112.0 * (e_launches + 1) / NB, 1), "wall_clock_value": round(all_pts / t_e2e_wall / 1e3, 2),
                     "launches": e_launches, "passes": e_passes, "pinned_on_numa_node": numa_node},
-            "gpu_launches": launches_per_pass * passes,
+            "gpu_launches": launches_per_pass * K,
             "clocks": sampler.summary(windows),
         }
         if cpu:

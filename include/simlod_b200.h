@@ -1,4 +1,4 @@
-// simlod_b200.h — C ABI of the B200-native SimLOD hot path.
+// simlod_b200.h — C ABI of the H100-native SimLOD hot path.
 //
 // The reference has no C library boundary: its host (modules/progressive_octree/
 // main_progressive_octree.cpp) compiles three CUDA programs at run time through
@@ -61,7 +61,7 @@ typedef struct SimlodConfig {
 } SimlodConfig;
 
 // initCuda + initCudaProgram (main.cpp:272-281, 549-642): context, streams, events, all device
-// buffers, the three programs (built-in sm_100a cubins), and a surface-capable RGBA8 array.
+// buffers, the three programs (built-in sm_90a cubins), and a surface-capable RGBA8 array.
 int  simlod_create(const SimlodConfig* config, SimlodContext** out);
 void simlod_destroy(SimlodContext* ctx);
 const char* simlod_last_error(void);

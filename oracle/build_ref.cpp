@@ -5,12 +5,12 @@
 // own run-time compilation pipeline:
 //   NVRTC per module with the reference's flag set  (include/CudaModularProgram.h:84-98)
 //   nvJitLink -dlto -arch=sm_<device>               (include/CudaModularProgram.h:214-239)
-// The reference does this at run time on the device it finds; there is no GPU in
-// the build container, so the link target is given on the command line (sm_100).
+// The reference does this at run time on the device it finds; the build needs no
+// GPU, so the link target is given on the command line (sm_90 for an H100).
 // No reference source is copied into this repository: the sources are read in
 // place and only the compiled cubins are written (oracle/_ref/ is git-ignored).
 //
-// usage: build_ref <reference_root> <out_dir> <sm_arch, e.g. 100>
+// usage: build_ref <reference_root> <out_dir> <sm_arch, e.g. 90>
 #include <cstdio>
 #include <cstdlib>
 #include <fstream>

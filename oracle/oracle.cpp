@@ -4,9 +4,9 @@
 //
 // Pinning (see oracle/README.md and DESIGN.md §6): the reference ships no tests, golden vectors or
 // fixtures (SURVEY.md §4), so this restatement is pinned against the reference's OWN kernels:
-//   * on the GPU box, tests/test_parity_gpu.py runs oracle/_ref/*.cubin (the unmodified reference
+//   * on the GPU, tests/test_parity_gpu.py compares with oracle/_ref/*.cubin (the unmodified reference
 //     sources compiled by oracle/build_ref.cpp) on the same inputs and compares canonical forms;
-//   * tests/golden/*.npz holds canonical digests produced by those reference kernels on a B200
+//   * tests/golden/*.npz holds canonical digests produced by those reference kernels on an H100
 //     (generator: tests/golden/make_golden.py); the CPU-only suite checks this file against them.
 //
 // The builder follows the reference phase by phase, serially:
@@ -16,7 +16,7 @@
 //   allocatePointChunks :485-538    allocateVoxelChunks :641-672
 //   insertPoints      :540-639      insertVoxels :674-698
 //   reset             reset.cu:20-86
-// Arithmetic follows the reference's SASS on sm_100 (see simlod_b200/csrc/fpmath.cuh): plain
+// Arithmetic follows the reference's SASS on sm_90 (see simlod_b200/csrc/fpmath.cuh): plain
 // mul/add/fma are IEEE round-to-nearest without flush; a/b is a*MUFU.RCP(b) with the product
 // flushed; float->uint saturates and flushes. MUFU.RCP cannot be reproduced on a CPU: it is exact
 // for powers of two (all CPU-only test cubes are 2^k); for other cube sizes the caller passes the

@@ -1,4 +1,4 @@
-"""simlod_b200 — B200-native (sm_100a) implementation of SimLOD's two hot paths.
+"""simlod_b200 — H100-native (sm_90a) implementation of SimLOD's two hot paths.
 
 Only what the path needs lives here:
   csrc/       hand-written CUDA kernels (kernel_construct, kernel_render, reset `kernel`) and the

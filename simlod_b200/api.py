@@ -13,7 +13,7 @@ observed through Stats):
     renderCUDA                   :465               render()
     stats read-back              :1201              stats()
 
-There is no fallback: if libsimlod_b200.so is missing or no B200 is present, construction raises.
+There is no fallback: if libsimlod_b200.so is missing or no H100 is present, construction raises.
 """
 import ctypes as C
 import os

@@ -1,12 +1,12 @@
 """Build recipe for the native parts (no torch involved).
 
-  simlod_b200/csrc/{construct,render,reset,util}.cu  --nvcc sm_100a-->  build/*.cubin
+  simlod_b200/csrc/{construct,render,reset,util}.cu  --nvcc sm_90a-->  build/*.cubin
   build/*.cubin --bin2c--> build/*_cubin.c  (embedded images)
   simlod_b200/csrc/host.cpp + images --g++--> simlod_b200/libsimlod_b200.so   (the C ABI, include/simlod_b200.h)
   build/*.cubin are also copied to simlod_b200/cubin/ : the drop-in artefacts for the reference's
   own host (INTEGRATION.md).
 
-The library is kept in-tree (git-ignored) so that it travels to the GPU box with the snapshot.
+The library is kept in-tree (git-ignored) so that the package imports from the source tree.
 """
 import os
 import shutil
@@ -24,7 +24,8 @@ CUBIN_DIR = os.path.join(ROOT, "simlod_b200", "cubin")
 PROGRAMS = ["construct", "render", "reset", "util", "las", "partition", "gen"]
 # gen.cu restates numpy generators in IEEE double arithmetic: no mul+add contraction
 EXTRA_FLAGS = {"gen": ["--fmad=false"]}
-ARCH = ["-gencode", "arch=compute_100a,code=sm_100a"]
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
+REF_ARCH = "90"
 
 
 def _run(cmd, **kw):
@@ -44,7 +45,7 @@ def _newer(target, sources):
 
 def _digest(paths, extra=""):
     """Content hash of the inputs of a build step: freshness must not depend on mtimes or on the intermediate
-    build/ directory, neither of which survives the trip to the GPU box (the built artefacts and the stamp do)."""
+    build/ directory, neither of which survives a copy of the tree to another machine (the built artefacts and the stamp do)."""
     import hashlib
     h = hashlib.sha256(extra.encode())
     for p in sorted(paths):
@@ -137,9 +138,13 @@ def build_oracle(force=False):
             po = os.path.join(ref_root, "modules", "progressive_octree")
             _run(["g++", "-O2", "-std=c++20", "-fPIC", "-shared", "-w", "-include", "cstdint", "-I" + po, "-I" + os.path.join(ref_root, "include"),
                   "-I" + os.path.join(ref_root, "libs", "fmt", "include"), os.path.join(po, "SimlodLoader.cpp"), shim2, "-o", sml, "-pthread"])
+        # the reference links for the device it runs on (sm_90 on an H100)
         outs = [os.path.join(refdir, n) for n in ("ref_construct.cubin", "ref_render.cubin", "ref_reset.cubin")]
-        if force or not all(os.path.exists(o) for o in outs):
-            _run([tool, ref_root, refdir, "100"], cwd=odir)
+        rstamp = os.path.join(refdir, "ref_cubins.stamp")
+        if force or not _stamp_matches(rstamp, REF_ARCH, outs):
+            _run([tool, ref_root, refdir, REF_ARCH], cwd=odir)
+            with open(rstamp, "w") as f:
+                f.write(REF_ARCH + "\n")
     return lib
 
 

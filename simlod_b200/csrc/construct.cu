@@ -1,4 +1,4 @@
-// construct.cu — incremental octree/LOD builder for sm_100a (B200).
+// construct.cu — incremental octree/LOD builder for sm_90a (H100).
 //
 // Drop-in for the reference's `kernel_construct`
 // (modules/progressive_octree/progressive_octree_voxels.cu:804-1010): same extern "C"
@@ -1492,7 +1492,7 @@ __device__ __noinline__ void insertAll(const Ctx c, const Batch b, uint32_t numS
 }
 
 // The control words every thread needs right after a grid barrier (this batch's counters, the clock, the heap mark, the
-// next batch's size). 4 736 warps loading the same few L2 lines one dependent load after the other cost several µs per
+// next batch's size). 4 224 warps (H100) loading the same few L2 lines one dependent load after the other serialise on every
 // batch; instead one thread per block loads all of them at once (independent loads, two of them 16 bytes wide) and the
 // block reads them from shared memory.
 struct Snapshot {

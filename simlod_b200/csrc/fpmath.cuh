@@ -2,7 +2,7 @@
 //
 // The reference kernels are NVRTC-compiled with --use_fast_math and then LTO-linked by
 // nvJitLink WITHOUT -ftz (include/CudaModularProgram.h:84-98,225). The SASS that results on
-// sm_100 (inspected with cuobjdump on oracle/_ref/*.cubin) therefore mixes
+// sm_90 (inspected with cuobjdump on oracle/_ref/*.cubin) therefore mixes
 //   * plain mul/add/fma  -> FMUL / FADD / FFMA     (round-to-nearest, denormals kept)
 //   * a / b              -> MUFU.RCP + FMUL.FTZ    (div.approx.ftz, front-end lowered)
 //   * pow(2, l)          -> MUFU.EX2               (ex2.approx.ftz)

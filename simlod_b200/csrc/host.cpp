@@ -5,7 +5,7 @@
 //   getUniforms                  :283-331        resetCUDA     :333-361
 //   updateOctree                 :364-428        renderCUDA    :465-546
 //   uploader step                :1033-1056      stats readback :1201-1216
-// The three programs are sm_100a cubins embedded in this library (the reference NVRTC-compiles
+// The three programs are sm_90a cubins embedded in this library (the reference NVRTC-compiles
 // its sources at start-up, CudaModularProgram.h:62-135); simlod_use_module swaps one of them
 // for an external cubin with the same kernel name (the reference's hot reload, :181-184).
 // There is no CPU fallback: without a device or a loadable cubin every call fails.
@@ -77,7 +77,7 @@ DriverApi drv;
 int loadDriver() {
     if (drv.loaded) return SIMLOD_OK;
     drv.handle = dlopen("libcuda.so.1", RTLD_NOW | RTLD_GLOBAL);
-    if (!drv.handle) return fail(SIMLOD_ERR_CUDA, "cannot load libcuda.so.1 (%s): a CUDA driver and a B200 are required, there is no CPU path", dlerror());
+    if (!drv.handle) return fail(SIMLOD_ERR_CUDA, "cannot load libcuda.so.1 (%s): a CUDA driver and an H100 are required, there is no CPU path", dlerror());
 #define X(name) drv.p_##name = reinterpret_cast<decltype(&name)>(dlsym(drv.handle, DRV_STR(name))); \
     if (!drv.p_##name) return fail(SIMLOD_ERR_CUDA, "libcuda.so.1 lacks %s", DRV_STR(name));
     DRV_LIST(X)
@@ -546,7 +546,7 @@ int simlod_get_uniforms(SimlodContext* ctx, SimlodUniforms* out) {
 
 int simlod_reset(SimlodContext* ctx) {
     // The reference launches the reset kernel with 1 block x 1 thread (main.cpp:348-354); one thread then zeroes the
-    // root's 256 KiB grid, 330 us on a B200. The kernel is grid-stride (reference reset.cu:78-85 and ours), so the
+    // root's 256 KiB grid alone. The kernel is grid-stride (reference reset.cu:78-85 and ours), so the
     // launch surface gives it one block per SM; simlod_reset_with_grid(ctx, 1, 1) is the reference's shape.
     if (!ctx) return fail(SIMLOD_ERR_INVALID, "null context");
     return simlod_reset_with_grid(ctx, (uint32_t)ctx->numSMs, 256);

@@ -17,7 +17,7 @@
 // Copy with non-temporal stores: the destination lines go to memory without being read or left in the cache.
 // The loaders must not fill the page-locked pool with ordinary stores (pread straight into it): each piece would
 // stay dirty in the cache of whichever core read it, and the copy engine's reads of such lines are served by
-// cross-core snoops — measured on the 2-socket host of the B200 box at ~19 GB/s against ~52 GB/s for lines that
+// cross-core snoops — measured on a 2-socket host at ~19 GB/s against ~52 GB/s for lines that
 // are in DRAM. Each loader therefore preads into a 256 KB cache-resident staging buffer and streams it out.
 static inline void copyStreaming(char* dst, const char* src, uint64_t bytes) {      // dst, src 16-byte aligned, bytes % 16 == 0
 #if defined(__x86_64__)

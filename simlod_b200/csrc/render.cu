@@ -1,4 +1,4 @@
-// render.cu — software point/voxel rasteriser for sm_100a (B200).
+// render.cu — software point/voxel rasteriser for sm_90a (H100).
 //
 // Drop-in for the reference's `kernel_render` (modules/progressive_octree/render.cu:1084-1355):
 // same extern "C" name and arguments, same outputs — Node::visible / Node::isLarge flags, the
@@ -335,8 +335,8 @@ __device__ void emitVisible(const EmitCtx& e, const uint32_t* visList, uint32_t 
     for (uint32_t v = warp; v < numVisible; v += numWarps) emitNode(e, &e.nodes[visList[v]]);
 }
 
-// one pass over the frame's items: every warp starts with the item of its own number (no atomic: 4 736 warps popping the
-// same counter at the same instant serialise for 10-20 us, a third of a small frame), then persistent warps pop the rest
+// one pass over the frame's items: every warp starts with the item of its own number (no atomic: 4 224 warps on an H100 popping the
+// same counter at the same instant would serialise), then persistent warps pop the rest
 // with a single atomicAdd each; a frame with no more items than warps touches the counter not at all.
 // (Measured and rejected, profiles/r02/render_notes.md: quarter-chunk items, 2 / 4 warps per item on small frames, the next
 // pop prefetched under the current item, four sample loads in flight per lane — each within 3 % of this loop or slower.)

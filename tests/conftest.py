@@ -9,7 +9,7 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a B200 (run with -m gpu on the GPU box)")
+    config.addinivalue_line("markers", "gpu: needs an H100 (run with -m gpu)")
 
 
 def _have_gpu():
@@ -39,7 +39,7 @@ def pytest_collection_modifyitems(config, items):
 @pytest.fixture(scope="session", autouse=True)
 def _native_built():
     """Build the native library and the oracle once (nvcc/g++ only; cross-compiles without a GPU).
-    On the GPU box the prebuilt artefacts travel with the snapshot and this is a no-op."""
+    Where build() has already run this is a no-op."""
     from simlod_b200 import build
     build.build_native()
     build.build_oracle()

@@ -1,14 +1,14 @@
-"""Generates tests/golden/reference_kernels_b200.npz ON THE GPU BOX by running the UNMODIFIED
-reference kernels (oracle/_ref/*.cubin = /root/reference sources compiled by oracle/build_ref.cpp
+"""Generates tests/golden/reference_kernels.npz on an H100 by running the UNMODIFIED
+reference kernels (oracle/_ref/*.cubin = the original sources compiled by oracle/build_ref.cpp
 with the reference's own NVRTC/nvJitLink recipe) through the headless launch surface:
 
-    gpurun -- python tests/golden/make_golden.py gpurun_out/reference_kernels_b200.npz
+    python tests/golden/make_golden.py <output .npz>
 
 For every case of tests/make_golden_cases.py it stores the canonical octree records, the
 deterministic Stats fields, MUFU.RCP(cube size) and the packed u64 framebuffer of one frame, all
 produced by the reference's kernel_construct / kernel / kernel_render. The CPU suite pins
-oracle/oracle.cpp (builder, canonicaliser and rasteriser) to these; the GPU suite does not read them:
-it runs the reference kernels live beside ours on the same buffers (tests/test_parity_gpu.py)."""
+oracle/oracle.cpp (builder, canonicaliser and rasteriser) to these; the GPU suite compares ours with
+the reference kernels on its own inputs (tests/test_parity_gpu.py, tests/reference_golden.py)."""
 import os
 import sys
 
@@ -50,4 +50,4 @@ def main(out):
 
 
 if __name__ == "__main__":
-    main(sys.argv[1] if len(sys.argv) > 1 else os.path.join(HERE, "reference_kernels_b200.npz"))
+    main(sys.argv[1] if len(sys.argv) > 1 else os.path.join(HERE, "reference_kernels.npz"))

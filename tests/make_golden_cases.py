@@ -1,5 +1,5 @@
-"""Inputs of the golden fixtures (shared by the generator, which runs the reference's kernels on a
-B200, and by the CPU-only test that checks the oracle against what they produced)."""
+"""Inputs of the golden fixtures (shared by the generator, which runs the reference's kernels on an
+H100, and by the CPU-only test that checks the oracle against what they produced)."""
 import numpy as np
 
 from simlod_b200 import camera, data

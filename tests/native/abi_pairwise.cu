@@ -1,53 +1,61 @@
-// Compile-time check of include/simlod_abi.h against the reference's OWN headers, field by field (run by
-// tests/test_abi_and_library.py with nvcc when /root/reference is present; nothing is executed).
+// Prints size and offset of every field of the host/device records, and the constants the kernels are built with,
+// one "Record.field offset size" line each. Built against include/simlod_abi.h (ours), or with -DSIMLOD_ABI_REFERENCE
+// against the reference's OWN headers (modules/progressive_octree); tests/test_abi_and_library.py requires the two
+// listings to be identical, the reference's being stored in tests/golden/reference.json.
 //   HostDeviceInterface.h  Uniforms, Stats, mat4     (host <-> device interface of the three kernels)
 //   structures.cuh         Point, Chunk, OccupancyGrid, Node and the constants the kernels are built with
 #include <cstddef>
 #include <cstdint>
-#include "HostDeviceInterface.h"      // reference (modules/progressive_octree)
+#include <cstdio>
+#ifdef SIMLOD_ABI_REFERENCE
+#include "HostDeviceInterface.h"      // reference
 #include "helper_math.h"              // reference: dot() used by structures.cuh
 #include "structures.cuh"             // reference
+typedef Point P; typedef Chunk Ch; typedef OccupancyGrid G; typedef Node N; typedef Uniforms U; typedef Stats S; typedef mat4 M;
+static const unsigned long long CONSTANTS[] = {MAX_POINTS_PER_NODE, POINTS_PER_CHUNK, MAX_DEPTH, GRID_NUM_CELLS / 32u, BATCH_STREAM_SIZE};
+#else
 #include "simlod_abi.h"               // ours
+typedef SimlodPoint P; typedef SimlodChunk Ch; typedef SimlodOccupancyGrid G; typedef SimlodNode N; typedef SimlodUniforms U;
+typedef SimlodStats S; typedef SimlodMat4 M;
+static const unsigned long long CONSTANTS[] = {SIMLOD_MAX_POINTS_PER_NODE, SIMLOD_POINTS_PER_CHUNK, SIMLOD_MAX_DEPTH, SIMLOD_GRID_WORDS,
+                                               SIMLOD_BATCH_STREAM_SIZE};
+#endif
 
-#define SAME_FIELD(OURS, REF, f) \
-    static_assert(offsetof(OURS, f) == offsetof(REF, f) && sizeof(((OURS*)nullptr)->f) == sizeof(((REF*)nullptr)->f), "layout of " #REF "::" #f)
+#define FIELD(T, f) std::printf("%s.%s %zu %zu\n", #T, #f, offsetof(T, f), sizeof(((T*)nullptr)->f))
 
-static_assert(sizeof(SimlodPoint) == sizeof(Point) && sizeof(SimlodChunk) == sizeof(Chunk) && sizeof(SimlodNode) == sizeof(Node), "record sizes");
-static_assert(sizeof(SimlodOccupancyGrid) == sizeof(OccupancyGrid) && sizeof(SimlodUniforms) == sizeof(Uniforms) && sizeof(SimlodStats) == sizeof(Stats), "record sizes");
-static_assert(sizeof(SimlodMat4) == sizeof(mat4), "mat4");
-static_assert(SIMLOD_MAX_POINTS_PER_NODE == MAX_POINTS_PER_NODE && SIMLOD_POINTS_PER_CHUNK == POINTS_PER_CHUNK && SIMLOD_MAX_DEPTH == MAX_DEPTH, "constants");
-static_assert(SIMLOD_GRID_WORDS == GRID_NUM_CELLS / 32u && SIMLOD_BATCH_STREAM_SIZE == BATCH_STREAM_SIZE, "constants");
+int main() {
+    std::printf("sizes %zu %zu %zu %zu %zu %zu %zu\n", sizeof(P), sizeof(Ch), sizeof(N), sizeof(G), sizeof(U), sizeof(S), sizeof(M));
+    std::printf("constants %llu %llu %llu %llu %llu\n", CONSTANTS[0], CONSTANTS[1], CONSTANTS[2], CONSTANTS[3], CONSTANTS[4]);
+    FIELD(P, x); FIELD(P, y); FIELD(P, z); FIELD(P, color);
+    FIELD(Ch, points); FIELD(Ch, size); FIELD(Ch, next);
+    FIELD(G, values);
 
-SAME_FIELD(SimlodPoint, Point, x); SAME_FIELD(SimlodPoint, Point, y); SAME_FIELD(SimlodPoint, Point, z); SAME_FIELD(SimlodPoint, Point, color);
-SAME_FIELD(SimlodChunk, Chunk, points); SAME_FIELD(SimlodChunk, Chunk, size); SAME_FIELD(SimlodChunk, Chunk, next);
-SAME_FIELD(SimlodOccupancyGrid, OccupancyGrid, values);
+    FIELD(N, children); FIELD(N, counter); FIELD(N, numPoints);
+    FIELD(N, level); FIELD(N, X); FIELD(N, Y); FIELD(N, Z);
+    FIELD(N, countIteration); FIELD(N, countFlag); FIELD(N, name);
+    FIELD(N, visible); FIELD(N, isFiltered); FIELD(N, isLeaf); FIELD(N, isLarge);
+    FIELD(N, grid); FIELD(N, points); FIELD(N, voxelChunks);
+    FIELD(N, numVoxels); FIELD(N, numVoxelsStored);
 
-SAME_FIELD(SimlodNode, Node, children); SAME_FIELD(SimlodNode, Node, counter); SAME_FIELD(SimlodNode, Node, numPoints);
-SAME_FIELD(SimlodNode, Node, level); SAME_FIELD(SimlodNode, Node, X); SAME_FIELD(SimlodNode, Node, Y); SAME_FIELD(SimlodNode, Node, Z);
-SAME_FIELD(SimlodNode, Node, countIteration); SAME_FIELD(SimlodNode, Node, countFlag); SAME_FIELD(SimlodNode, Node, name);
-SAME_FIELD(SimlodNode, Node, visible); SAME_FIELD(SimlodNode, Node, isFiltered); SAME_FIELD(SimlodNode, Node, isLeaf); SAME_FIELD(SimlodNode, Node, isLarge);
-SAME_FIELD(SimlodNode, Node, grid); SAME_FIELD(SimlodNode, Node, points); SAME_FIELD(SimlodNode, Node, voxelChunks);
-SAME_FIELD(SimlodNode, Node, numVoxels); SAME_FIELD(SimlodNode, Node, numVoxelsStored);
+    FIELD(U, width); FIELD(U, height); FIELD(U, time);
+    FIELD(U, fovy_rad); FIELD(U, world); FIELD(U, view);
+    FIELD(U, proj); FIELD(U, transform); FIELD(U, transform_updateBound);
+    FIELD(U, transformInv_updateBound); FIELD(U, persistentBufferCapacity);
+    FIELD(U, momentaryBufferCapacity); FIELD(U, frameCounter);
+    FIELD(U, boxMin); FIELD(U, boxMax);
+    FIELD(U, showBoundingBox); FIELD(U, showPoints); FIELD(U, colorByNode);
+    FIELD(U, colorByLOD); FIELD(U, colorWhite); FIELD(U, doUpdateVisibility);
+    FIELD(U, doProgressive); FIELD(U, LOD); FIELD(U, useHighQualityShading);
+    FIELD(U, minNodeSize); FIELD(U, pointSize); FIELD(U, updateStats);
+    FIELD(U, enableEDL); FIELD(U, edlStrength);
 
-SAME_FIELD(SimlodUniforms, Uniforms, width); SAME_FIELD(SimlodUniforms, Uniforms, height); SAME_FIELD(SimlodUniforms, Uniforms, time);
-SAME_FIELD(SimlodUniforms, Uniforms, fovy_rad); SAME_FIELD(SimlodUniforms, Uniforms, world); SAME_FIELD(SimlodUniforms, Uniforms, view);
-SAME_FIELD(SimlodUniforms, Uniforms, proj); SAME_FIELD(SimlodUniforms, Uniforms, transform); SAME_FIELD(SimlodUniforms, Uniforms, transform_updateBound);
-SAME_FIELD(SimlodUniforms, Uniforms, transformInv_updateBound); SAME_FIELD(SimlodUniforms, Uniforms, persistentBufferCapacity);
-SAME_FIELD(SimlodUniforms, Uniforms, momentaryBufferCapacity); SAME_FIELD(SimlodUniforms, Uniforms, frameCounter);
-SAME_FIELD(SimlodUniforms, Uniforms, boxMin); SAME_FIELD(SimlodUniforms, Uniforms, boxMax);
-SAME_FIELD(SimlodUniforms, Uniforms, showBoundingBox); SAME_FIELD(SimlodUniforms, Uniforms, showPoints); SAME_FIELD(SimlodUniforms, Uniforms, colorByNode);
-SAME_FIELD(SimlodUniforms, Uniforms, colorByLOD); SAME_FIELD(SimlodUniforms, Uniforms, colorWhite); SAME_FIELD(SimlodUniforms, Uniforms, doUpdateVisibility);
-SAME_FIELD(SimlodUniforms, Uniforms, doProgressive); SAME_FIELD(SimlodUniforms, Uniforms, LOD); SAME_FIELD(SimlodUniforms, Uniforms, useHighQualityShading);
-SAME_FIELD(SimlodUniforms, Uniforms, minNodeSize); SAME_FIELD(SimlodUniforms, Uniforms, pointSize); SAME_FIELD(SimlodUniforms, Uniforms, updateStats);
-SAME_FIELD(SimlodUniforms, Uniforms, enableEDL); SAME_FIELD(SimlodUniforms, Uniforms, edlStrength);
-
-SAME_FIELD(SimlodStats, Stats, frameID); SAME_FIELD(SimlodStats, Stats, numNodes); SAME_FIELD(SimlodStats, Stats, numInner); SAME_FIELD(SimlodStats, Stats, numLeaves);
-SAME_FIELD(SimlodStats, Stats, numNonemptyLeaves); SAME_FIELD(SimlodStats, Stats, numPoints); SAME_FIELD(SimlodStats, Stats, numVoxels);
-SAME_FIELD(SimlodStats, Stats, allocatedBytes_momentary); SAME_FIELD(SimlodStats, Stats, allocatedBytes_persistent);
-SAME_FIELD(SimlodStats, Stats, numVisibleNodes); SAME_FIELD(SimlodStats, Stats, numVisibleInner); SAME_FIELD(SimlodStats, Stats, numVisibleLeaves);
-SAME_FIELD(SimlodStats, Stats, numVisiblePoints); SAME_FIELD(SimlodStats, Stats, numVisibleVoxels); SAME_FIELD(SimlodStats, Stats, numChunksPoints);
-SAME_FIELD(SimlodStats, Stats, numChunksVoxels); SAME_FIELD(SimlodStats, Stats, batchletIndex); SAME_FIELD(SimlodStats, Stats, numPointsProcessed);
-SAME_FIELD(SimlodStats, Stats, numAllocatedChunks); SAME_FIELD(SimlodStats, Stats, chunkPoolSize); SAME_FIELD(SimlodStats, Stats, dbg);
-SAME_FIELD(SimlodStats, Stats, memCapacityReached);
-
-int main() { return 0; }
+    FIELD(S, frameID); FIELD(S, numNodes); FIELD(S, numInner); FIELD(S, numLeaves);
+    FIELD(S, numNonemptyLeaves); FIELD(S, numPoints); FIELD(S, numVoxels);
+    FIELD(S, allocatedBytes_momentary); FIELD(S, allocatedBytes_persistent);
+    FIELD(S, numVisibleNodes); FIELD(S, numVisibleInner); FIELD(S, numVisibleLeaves);
+    FIELD(S, numVisiblePoints); FIELD(S, numVisibleVoxels); FIELD(S, numChunksPoints);
+    FIELD(S, numChunksVoxels); FIELD(S, batchletIndex); FIELD(S, numPointsProcessed);
+    FIELD(S, numAllocatedChunks); FIELD(S, chunkPoolSize); FIELD(S, dbg);
+    FIELD(S, memCapacityReached);
+    return 0;
+}

@@ -47,11 +47,11 @@ def test_library_exports_every_declared_symbol():
     assert set(declared) <= exported
 
 
-def test_cubins_are_sm100a_and_export_reference_kernel_names():
+def test_cubins_are_sm90a_and_export_reference_kernel_names():
     for prog, kernel in (("construct", "kernel_construct"), ("render", "kernel_render"), ("reset", "kernel")):
         path = os.path.join(ROOT, "simlod_b200", "cubin", "simlod_%s.cubin" % prog)
         out = subprocess.check_output(["cuobjdump", "-elf", path], text=True, stderr=subprocess.STDOUT)
-        assert "sm_100a" in out or "SM100a" in out or "EF_CUDA_SM100" in out, out[:400]
+        assert ".target sm_90a" in out, out[:400]
         syms = subprocess.check_output(["cuobjdump", "-symbols", path], text=True, stderr=subprocess.STDOUT)
         assert re.search(r"STT_FUNC\s+STB_GLOBAL\s+\S+\s+%s\b" % kernel, syms) or (" %s" % kernel) in syms
 
@@ -91,15 +91,17 @@ def test_generators_are_counter_based():
 
 
 def test_abi_matches_the_reference_headers_field_by_field(tmp_path):
-    """tests/native/abi_pairwise.cu includes the reference's OWN HostDeviceInterface.h / structures.cuh next to
-    include/simlod_abi.h and static_asserts size and offset of every field pairwise (compile-only)."""
-    import shutil
-    import subprocess
-    ref = os.environ.get("SIMLOD_REFERENCE", "/root/reference")
-    po = os.path.join(ref, "modules", "progressive_octree")
-    if not os.path.isdir(po) or shutil.which("nvcc") is None:
-        pytest.skip("needs the reference tree and nvcc (build-time check; the GPU box has neither mounted)")
-    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    r = subprocess.run(["nvcc", "-std=c++17", "-c", "-o", str(tmp_path / "abi_pairwise.o"), "-I" + po, "-I" + os.path.join(root, "include"),
-                        os.path.join(root, "tests", "native", "abi_pairwise.cu")], capture_output=True, text=True, timeout=600)
-    assert r.returncode == 0, r.stderr[-2000:]
+    """tests/native/abi_pairwise.cu lists size and offset of every field of include/simlod_abi.h; the same listing of the
+    reference's OWN HostDeviceInterface.h / structures.cuh (stored in tests/golden/reference.json) must be identical."""
+    import reference_golden as golden
+    src = os.path.join(ROOT, "tests", "native", "abi_pairwise.cu")
+
+    def listing(cmd):
+        subprocess.check_call(cmd + ["-o", str(tmp_path / "abi"), src])
+        return subprocess.check_output([str(tmp_path / "abi")], text=True).splitlines()
+
+    def reference():
+        po = os.path.join(os.environ["SIMLOD_REFERENCE"], "modules", "progressive_octree")     # the original SimLOD sources
+        return {"layout": listing(["nvcc", "-std=c++17", "-DSIMLOD_ABI_REFERENCE", "-I" + po])}
+    ours = {"layout": listing(["g++", "-std=c++17", "-x", "c++", "-I" + os.path.join(ROOT, "include")])}
+    golden.assert_same(ours, golden.reference("abi_layout", reference), "include/simlod_abi.h vs the reference headers")

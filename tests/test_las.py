@@ -1,15 +1,12 @@
 """LAS front-end row (SURVEY.md §8f-2): record decode. CPU part pins the oracle against the reference's
-own LasLoader.cpp (compiled into oracle/_ref/libref_las.so); GPU part pins our device decode against both."""
-import os
-
+own LasLoader.cpp (oracle/_ref/libref_las.so, its results stored in tests/golden/reference.json); GPU part pins our
+device decode against both."""
 import numpy as np
 import pytest
 
 import oracle
+import reference_golden as golden
 from simlod_b200 import data
-
-HAVE_REF_LAS = os.path.exists(oracle.REF_LAS_LIB)
-needs_ref_las = pytest.mark.skipif(not HAVE_REF_LAS, reason="oracle/_ref/libref_las.so not built (needs /root/reference at build time)")
 
 SCALE = (0.001, 0.002, 0.0005)
 OFFSET = (10.0, -5.0, 2.5)
@@ -24,7 +21,11 @@ def same_points(a, b, with_color=True):
     return bool(ok)
 
 
-@needs_ref_las
+def reference_las(path, first, count, fmt, key):
+    """What the reference's LasLoader.cpp reads from `path` (golden.points, colour compared for the RGB formats)."""
+    return golden.reference(key, lambda: golden.points(oracle.ref_las_load(path, first, count, TRANSLATION), fmt in (2, 3, 5, 7)))
+
+
 @pytest.mark.parametrize("fmt,wide,extra", [(2, True, 0), (2, False, 0), (3, True, 0), (0, True, 0), (1, True, 0),
                                             (5, True, 0), (7, True, 0), (2, True, 1), (3, False, 3)])      # 5: 63-byte records; odd extra bytes
 def test_oracle_decode_matches_reference_lasloader(tmp_path, fmt, wide, extra):
@@ -32,9 +33,9 @@ def test_oracle_decode_matches_reference_lasloader(tmp_path, fmt, wide, extra):
     path = str(tmp_path / "t.las")
     rec = data.write_las(path, pts, fmt=fmt, scale=SCALE, offset=OFFSET, wide_colors=wide, extra_bytes=extra)
     for first, count in ((0, 60_000), (123, 4_567), (59_999, 1)):
-        ref = oracle.ref_las_load(path, first, count, TRANSLATION)
+        ref = reference_las(path, first, count, fmt, "las/cpu/fmt%d/wide%d/extra%d/%d+%d" % (fmt, wide, extra, first, count))
         got = oracle.decode_las(rec[first:first + count], count, rec.shape[1], fmt, SCALE, OFFSET, TRANSLATION)
-        assert same_points(ref, got, with_color=fmt in (2, 3, 5, 7)), (fmt, first, count)
+        golden.assert_same(golden.points(got, fmt in (2, 3, 5, 7)), ref, "fmt %d, points %d + %d" % (fmt, first, count))
 
 
 def test_decode_roundtrip_properties():
@@ -69,9 +70,9 @@ def test_device_decode_matches_oracle_and_reference(tmp_path, fmt, extra):
             got = sim.ring_slot(slot, n)
             want = oracle.decode_las(rec[first:first + n], n, rec.shape[1], fmt, SCALE, OFFSET, TRANSLATION)
             assert same_points(got, want, with_color=True), (fmt, slot)
-            if HAVE_REF_LAS and n:
-                ref = oracle.ref_las_load(path, first, n, TRANSLATION)
-                assert same_points(got, ref, with_color=fmt in (2, 3, 5, 7)), (fmt, slot)
+            if n:
+                ref = reference_las(path, first, n, fmt, "las/device/fmt%d/extra%d/%d+%d" % (fmt, extra, first, n))
+                golden.assert_same(golden.points(got, fmt in (2, 3, 5, 7)), ref, "fmt %d, slot %d" % (fmt, slot))
             first += n
     finally:
         sim.close()

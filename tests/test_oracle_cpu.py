@@ -1,6 +1,6 @@
 """CPU-only checks of the oracle (oracle/oracle.cpp) against independent restatements and against
 properties the reference's algorithm guarantees, plus the golden digests produced by the
-reference's own kernels on a B200 (tests/golden/, see make_golden.py)."""
+reference's own kernels on an H100 (tests/golden/, see make_golden.py)."""
 import os
 
 import numpy as np
@@ -166,10 +166,10 @@ def test_out_of_box_points_follow_the_reference_quirks():
     assert leaves["numPoints"].sum() == 60_000
 
 
-GOLDEN = os.path.join(os.path.dirname(__file__), "golden", "reference_kernels_b200.npz")
+GOLDEN = os.path.join(os.path.dirname(__file__), "golden", "reference_kernels.npz")
 
 
-@pytest.mark.skipif(not os.path.exists(GOLDEN), reason="golden digests not generated yet (tests/golden/make_golden.py on the GPU box)")
+@pytest.mark.skipif(not os.path.exists(GOLDEN), reason="golden digests not generated yet (tests/golden/make_golden.py on a GPU)")
 def test_oracle_matches_golden_digests_from_the_reference_kernels():
     import make_golden_cases as cases
     g = np.load(GOLDEN)

@@ -1,29 +1,27 @@
-"""GPU parity tests (run on the B200 box with -m gpu). Everything goes through the C ABI.
+"""GPU parity tests (run with -m gpu on an H100). Everything goes through the C ABI.
 
 Three-way comparison on the same inputs:
-  ours (built-in sm_100a cubins)  vs  CPU oracle (oracle/oracle.cpp)  vs  the reference's own
-  kernels (oracle/_ref/*.cubin, compiled from /root/reference by oracle/build_ref.cpp).
-Integer/byte results are compared bit-exactly on the canonical form (DESIGN.md §3); the
-framebuffer is compared as raw u64 words with both rasterisers fed the identical octree buffers.
+  ours (built-in sm_90a cubins)  vs  CPU oracle (oracle/oracle.cpp)  vs  the reference's own
+  kernels (oracle/_ref/*.cubin, compiled from the original sources by oracle/build_ref.cpp), whose
+  results are stored as digests in tests/golden/reference.json (tests/reference_golden.py).
+Integer/byte results are compared bit-exactly on the canonical form (DESIGN.md §3). A frame is compared by the
+depth word of every pixel, the visible counts and the per-node visibility flags; when it draws no voxel, also as
+raw u64 framebuffer words and RGBA8 surface bytes (voxel colours are a race in the builders: reference_golden.frame).
 """
-import os
-
 import numpy as np
 import pytest
 
 import oracle
+import reference_golden as golden
 from simlod_b200 import SimLOD, camera, data
 
 pytestmark = pytest.mark.gpu
-
-HAVE_REF = all(os.path.exists(p) for p in oracle.REF_CUBINS.values())
-needs_ref = pytest.mark.skipif(not HAVE_REF, reason="oracle/_ref/*.cubin not built (needs /root/reference at build time)")
 
 
 @pytest.fixture(scope="module")
 def sim():
     # 3 render blocks per SM = the grid the reference's own kernel gets from the occupancy query on
-    # sm_100 (72 registers); EDL tile coverage depends on the grid size (render.cu:1273)
+    # sm_90 (80 registers); EDL tile coverage depends on the grid size (render.cu:1273)
     s = SimLOD(1920, 1080, momentary_bytes=oracle.REF_MOMENTARY_BYTES, persistent_bytes=12 << 30, render_blocks_per_sm=3)
     yield s
     s.close()
@@ -43,6 +41,11 @@ def build_gpu(sim, batches, box, reference=False):
     canon = oracle.canon_from_image(*sim.download_octree())
     use_reference(sim, (0, 2), False)
     return stats, canon
+
+
+def reference_octree(sim, key, batches, box):
+    """The reference kernels' octree of `batches` (golden.octree)."""
+    return golden.reference(key, lambda: golden.octree(*build_gpu(sim, batches, box, reference=True)))
 
 
 def build_oracle(batches, box, rcp=0.0):
@@ -77,15 +80,18 @@ def test_config1_uniform_1m_single_batch_vs_oracle(sim):
     assert o.check_voxel_colors(cn) == 0
 
 
-@needs_ref
 def test_config1_uniform_1m_single_batch_vs_reference_kernels(sim):
     pts, mn, mx = data.uniform_cube(1_000_000)
     st, cn = build_gpu(sim, [pts], (mn, mx))
-    st_r, cn_r = build_gpu(sim, [pts], (mn, mx), reference=True)
-    assert_same_octree(st, cn, st_r, cn_r, "ours vs reference kernels")
     o = build_oracle([pts], (mn, mx))
-    assert_same_octree(st_r, cn_r, o.stats(), o.canon(), "reference kernels vs oracle")
-    assert o.check_voxel_colors(cn_r) == 0
+
+    def run():          # the reference's octree, and the voxel colours of it the oracle rejects
+        st_r, cn_r = build_gpu(sim, [pts], (mn, mx), reference=True)
+        return dict(golden.octree(st_r, cn_r), voxel_color_errors=int(o.check_voxel_colors(cn_r)))
+    ref = golden.reference("config1_uniform_1m", run)
+    golden.assert_same(golden.octree(st, cn), ref, "ours vs reference kernels")
+    golden.assert_same(golden.octree(o.stats(), o.canon()), ref, "reference kernels vs oracle")
+    assert ref["voxel_color_errors"] == 0
 
 
 TERRAIN_N = 3_300_000
@@ -108,12 +114,10 @@ def test_streamed_ragged_batches_vs_oracle(sim):
     assert o.check_voxel_colors(cn) == 0
 
 
-@needs_ref
 def test_streamed_ragged_batches_vs_reference_kernels(sim):
     batches, box = terrain_batches()
     st, cn = build_gpu(sim, batches, box)
-    st_r, cn_r = build_gpu(sim, batches, box, reference=True)
-    assert_same_octree(st, cn, st_r, cn_r, "ours vs reference kernels")
+    golden.assert_same(golden.octree(st, cn), reference_octree(sim, "terrain_ragged", batches, box), "ours vs reference kernels")
 
 
 def test_small_batches_grow_a_leaf_root_then_split(sim):
@@ -126,13 +130,11 @@ def test_small_batches_grow_a_leaf_root_then_split(sim):
     assert o.check_voxel_colors(cn) == 0
 
 
-@needs_ref
 def test_small_batches_vs_reference_kernels(sim):
     pts, mn, mx = data.uniform_cube(120_000, size=64.0, seed=5)
     batches = split(pts, [20_000, 20_000, 10_000, 1, 30_000, 39_999])
     st, cn = build_gpu(sim, batches, (mn, mx))
-    st_r, cn_r = build_gpu(sim, batches, (mn, mx), reference=True)
-    assert_same_octree(st, cn, st_r, cn_r, "ours vs reference kernels")
+    golden.assert_same(golden.octree(st, cn), reference_octree(sim, "small_batches", batches, (mn, mx)), "ours vs reference kernels")
 
 
 def test_leaf_capacity_is_inclusive_and_out_of_box_points_are_mirrored(sim):
@@ -173,17 +175,32 @@ def cameras(box_size, w, h):
     yield "inside", camera.orbit_camera(2.2, 0.1, r * 0.01, (box_size[0] * 0.5, box_size[1] * 0.5, box_size[2] * 0.5), w, h)
 
 
-def render_both(sim):
-    out = {}
-    for ref in (False, True):
-        use_reference(sim, (1,), ref)
-        sim.render()
-        out[ref] = (sim.framebuffer(), sim.surface(), sim.stats(), sim.memcpy_dtoh(sim.buffers().nodes, sim.stats().numNodes * 152))
-    use_reference(sim, (1,), False)
-    return out
+VISIBLE = ("numVisibleNodes", "numVisibleInner", "numVisibleLeaves", "numVisiblePoints", "numVisibleVoxels")
 
 
-@needs_ref
+def render_frame(sim):
+    """One frame: (golden.frame digest with the per-node visibility flags, raw framebuffer, Stats)."""
+    sim.render()
+    st = sim.stats()
+    fb = sim.framebuffer()
+    nodes = sim.memcpy_dtoh(sim.buffers().nodes, st.numNodes * 152)
+    return golden.frame(fb, sim.surface(), [getattr(st, f) for f in VISIBLE], st.numVisibleVoxels, nodes), fb, st
+
+
+def render_vs_reference(sim, key, label):
+    """Our frame against the reference kernel's frame of the same octree and Uniforms (reference_golden.frame)."""
+    ours, fb, st = render_frame(sim)
+
+    def run():
+        use_reference(sim, (1,), True)
+        try:
+            return render_frame(sim)[0]
+        finally:
+            use_reference(sim, (1,), False)
+    golden.assert_same(ours, golden.reference(key, run), label)
+    return fb, st
+
+
 @pytest.mark.parametrize("hqs", [0, 1])
 @pytest.mark.parametrize("dataset", ["uniform", "terrain"])
 def test_framebuffer_bit_exact_vs_reference_kernel(sim, dataset, hqs):
@@ -197,20 +214,10 @@ def test_framebuffer_bit_exact_vs_reference_kernel(sim, dataset, hqs):
     sim.set_settings(useHighQualityShading=hqs, pointSize=1)
     for name, (view, proj) in cameras(mx, sim.width, sim.height):
         sim.set_camera(view, proj)
-        r = render_both(sim)
-        (fb_o, su_o, st_o, nodes_o), (fb_r, su_r, st_r, nodes_r) = r[False], r[True]
-        flags_o = nodes_o.reshape(-1, 152)[:, [116, 119]]
-        flags_r = nodes_r.reshape(-1, 152)[:, [116, 119]]
-        assert (flags_o == flags_r).all(), "%s: %d visibility flags differ" % (name, int((flags_o != flags_r).sum()))
-        for f in ("numVisibleNodes", "numVisibleInner", "numVisibleLeaves", "numVisiblePoints", "numVisibleVoxels"):
-            assert getattr(st_o, f) == getattr(st_r, f), (name, f)
-        assert ((fb_o >> np.uint64(32)) == (fb_r >> np.uint64(32))).all(), "%s: depth words differ" % name
-        assert (fb_o == fb_r).all(), "%s: %d framebuffer words differ" % (name, int((fb_o != fb_r).sum()))
-        assert (su_o == su_r).all(), "%s: surface differs" % name
+        render_vs_reference(sim, "frame/%s/hqs%d/%s" % (dataset, hqs, name), name)
     sim.set_settings(useHighQualityShading=0)
 
 
-@needs_ref
 def test_framebuffer_point_size_2_and_lod_colours(sim):
     pts, mn, mx = data.terrain(2_000_000)
     build_gpu(sim, list(data.batches(pts)), (mn, mx))
@@ -220,12 +227,10 @@ def test_framebuffer_point_size_2_and_lod_colours(sim):
                      dict(colorByNode=1), dict(colorByNode=1, colorByLOD=1), dict(colorByNode=1, useHighQualityShading=1)):     # render.cu:73-78
         sim.set_settings(pointSize=1, colorByLOD=0, colorByNode=0, useHighQualityShading=0)
         sim.set_settings(**settings)
-        r = render_both(sim)
-        assert (r[False][0] == r[True][0]).all(), settings
+        render_vs_reference(sim, "frame/settings/" + ",".join("%s=%d" % kv for kv in sorted(settings.items())), repr(settings))
     sim.set_settings(pointSize=1, colorByLOD=0, colorByNode=0, useHighQualityShading=0)
 
 
-@needs_ref
 def test_framebuffer_with_frozen_visibility_transform(sim):
     # settings.doUpdateVisibility off (main.cpp:300-306): the LOD cut keeps the bound transform of the previous view
     # (transform_updateBound, render.cu:792-852) while the samples are splatted with the new one (transform, render.cu:62)
@@ -239,15 +244,11 @@ def test_framebuffer_with_frozen_visibility_transform(sim):
         sim.set_settings(useHighQualityShading=hqs)
         sim.set_camera(*far)
         sim.set_camera(*close, update_visibility=False)
-        frozen = render_both(sim)
-        assert (frozen[False][3].reshape(-1, 152)[:, [116, 119]] == frozen[True][3].reshape(-1, 152)[:, [116, 119]]).all()
-        assert (frozen[False][0] == frozen[True][0]).all(), "frozen visibility transform, hqs %d" % hqs
-        assert (frozen[False][1] == frozen[True][1]).all()
-        assert frozen[False][2].numVisibleVoxels > 0 and frozen[False][2].numVisiblePoints == 0      # the far cut, seen from close
+        frozen_fb, frozen_st = render_vs_reference(sim, "frame/frozen/hqs%d" % hqs, "frozen visibility transform, hqs %d" % hqs)
+        assert frozen_st.numVisibleVoxels > 0 and frozen_st.numVisiblePoints == 0      # the far cut, seen from close
         sim.set_camera(*close)
-        moved = render_both(sim)
-        assert (moved[False][0] == moved[True][0]).all()
-        assert (frozen[False][0] != moved[False][0]).any()
+        moved_fb, _ = render_vs_reference(sim, "frame/moved/hqs%d" % hqs, "moved, hqs %d" % hqs)
+        assert (frozen_fb != moved_fb).any()
     sim.set_settings(useHighQualityShading=0)
 
 
@@ -257,11 +258,20 @@ def cache_counters(sim):
     return int(c[0]), int(c[1])
 
 
-@needs_ref
+def scribble_over_the_chunk_list_cache(sim, seed):
+    """Seeded garbage over the tail of the render buffer that holds the chunk-list cache (render.cu, behind the HQS targets
+    of this resolution), as another kernel using the buffer as scratch would leave it."""
+    px = sim.width * sim.height
+    color = 31200144 + ((px * 8 + 15) & ~15) + 16 + ((px * 4 + 15) & ~15)
+    off = (color + 16 * px + 255) & ~255
+    junk = np.random.default_rng(seed).integers(0, 256, 200_000_000 - off, dtype=np.uint8)
+    sim.memcpy_htod(sim.buffers().renderbuffer + off, junk)
+
+
 def test_chunk_list_cache_is_only_a_hint(sim):
     """The rasteriser keeps the chunk pointers of drawn nodes across frames and verifies them against the octree before
     use. Frames must equal the reference kernel's whatever happens between them: growth of the lists, a reset followed by
-    a different octree at the same addresses, and another render kernel using the buffer as scratch."""
+    a different octree at the same addresses, and other contents left in the buffer."""
     pts, mn, mx = data.terrain(5_000_000)
     batches = list(data.batches(pts))
     sim.set_settings(pointSize=1, colorByLOD=0, colorByNode=0, useHighQualityShading=0)
@@ -269,9 +279,7 @@ def test_chunk_list_cache_is_only_a_hint(sim):
     sim.set_camera(view, proj)
 
     def same_as_reference(label):
-        r = render_both(sim)                       # ours, then the reference kernel (which scribbles over the buffer)
-        assert (r[False][0] == r[True][0]).all(), label
-        return r[False][0]
+        return render_vs_reference(sim, "cache/" + label, label)[0]
 
     build_gpu(sim, batches[:3], (mn, mx))
     a = same_as_reference("first frame")
@@ -279,7 +287,8 @@ def test_chunk_list_cache_is_only_a_hint(sim):
     hits, walks = cache_counters(sim)
     assert hits > 0 and walks == 0, (hits, walks)                        # second frame in a row: every list comes from the cache
     assert (sim.framebuffer() == a).all()
-    same_as_reference("after the reference kernel used the buffer")     # its scratch overwrote ours: verified, rebuilt
+    scribble_over_the_chunk_list_cache(sim, 1)
+    same_as_reference("after the buffer was overwritten")               # garbage in the cache: verified, rebuilt
     # the lists grow: two more batches into the same octree
     for b in batches[3:]:
         sim.upload_batch(b)
@@ -458,10 +467,8 @@ def test_spill_buffer_overflow_postpones_splits_and_loses_nothing(sim):
         assert (cn.records["level"] <= 4).all()
 
 
-@needs_ref
 def test_shell_stream_vs_reference_kernels(sim):
     pts, mn, mx = data.shell(2_400_000)
     batches = list(data.batches(pts))
     st, cn = build_gpu(sim, batches, (mn, mx))
-    st_r, cn_r = build_gpu(sim, batches, (mn, mx), reference=True)
-    assert_same_octree(st, cn, st_r, cn_r, "shell: ours vs reference kernels")
+    golden.assert_same(golden.octree(st, cn), reference_octree(sim, "shell", batches, (mn, mx)), "shell: ours vs reference kernels")

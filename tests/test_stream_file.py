@@ -1,17 +1,16 @@
-"""Streaming front-end row (SURVEY.md §8f-1): .simlod container, the reference's own loader as CPU reference,
-and (GPU) the file streamer: header -> box, reset, loader threads + pinned pool + in-order upload."""
+"""Streaming front-end row (SURVEY.md §8f-1): .simlod container, the reference's own loader as CPU reference
+(its results stored in tests/golden/reference.json), and (GPU) the file streamer: header -> box, reset, loader threads +
+pinned pool + in-order upload."""
 import os
 
 import numpy as np
 import pytest
 
 import oracle
+import reference_golden as golden
 from simlod_b200 import data
 
-needs_ref = pytest.mark.skipif(not os.path.exists(oracle.REF_SIMLOD_LIB), reason="oracle/_ref/libref_simlod.so not built")
 
-
-@needs_ref
 def test_simlod_container_roundtrip_through_reference_loader(tmp_path):
     pts, mn, mx = data.terrain(123_457)
     path = str(tmp_path / "t.simlod")
@@ -20,8 +19,9 @@ def test_simlod_container_roundtrip_through_reference_loader(tmp_path):
     hdr = np.fromfile(path, dtype="<f4", count=6)
     assert np.allclose(hdr[:3], mn) and np.allclose(hdr[3:], mx)
     for first, count in ((0, 123_457), (100_000, 23_457), (5, 1)):
-        got = oracle.ref_simlod_load(path, first, count)           # loadFileNative, SimlodLoader.cpp:147-157
-        assert (got == pts[first:first + count]).all()
+        got = golden.reference("simlod/%d+%d" % (first, count),                 # loadFileNative, SimlodLoader.cpp:147-157
+                               lambda: {"points": golden.sha256(oracle.ref_simlod_load(path, first, count))})
+        golden.assert_same({"points": golden.sha256(pts[first:first + count])}, got, "points %d + %d" % (first, count))
 
 
 @pytest.mark.gpu

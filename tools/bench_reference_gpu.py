@@ -1,6 +1,6 @@
 """Developer tool (not part of bench.py): times the reference's OWN kernels (oracle/_ref/*.cubin) on
-the same B200, same harness, same inputs as bench.py's workload — the "R-GPU" baseline of
-BASELINE.md §2. Writes one JSON object; the committed copy lives in profiles/."""
+the same H100, same harness, same inputs as bench.py's workload — the "R-GPU" baseline of
+BASELINE.md §2. Writes one JSON object."""
 import json
 import os
 import sys

@@ -108,7 +108,7 @@ for name, batches, box, rcp in cases:
 import subprocess  # noqa: E402
 timed = os.path.join(ROOT, "tools", "exp", "dev_timers2.cubin")
 os.makedirs(os.path.dirname(timed), exist_ok=True)
-r = subprocess.run(["nvcc", "-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-std=c++17", "-lineinfo", "-cubin", "-DSIMLOD_TIMERS=2", "-o", timed,
+r = subprocess.run(["nvcc", "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-std=c++17", "-lineinfo", "-cubin", "-DSIMLOD_TIMERS=2", "-o", timed,
                     os.path.join(ROOT, "simlod_b200", "csrc", "construct.cu")], capture_output=True, text=True)
 if r.returncode != 0:
     print("timers build failed:", r.stderr[-300:]); timed = None

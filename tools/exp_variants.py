@@ -45,7 +45,7 @@ for name, flags in KNOBS.items():
         if stale != out:
             os.remove(stale)
     if not os.path.exists(out):
-        cmd = ["nvcc", "-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-std=c++17", "-lineinfo", "-cubin"] + flags + \
+        cmd = ["nvcc", "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-std=c++17", "-lineinfo", "-cubin"] + flags + \
               ["-o", out, os.path.join(ROOT, "simlod_b200", "csrc", "construct.cu")]
         r = subprocess.run(cmd, capture_output=True, text=True)
         if r.returncode != 0:

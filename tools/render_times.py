@@ -27,7 +27,7 @@ NAMES = ["clear|vis+cut", "-", "items", "draw", "stats+edl"]
 import subprocess  # noqa: E402
 timed = os.path.join(ROOT, "tools", "exp", "render_timers.cubin")
 os.makedirs(os.path.dirname(timed), exist_ok=True)
-r = subprocess.run(["nvcc", "-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-std=c++17", "-lineinfo", "-cubin", "-DSIMLOD_RENDER_TIMERS=1", "-o", timed,
+r = subprocess.run(["nvcc", "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-std=c++17", "-lineinfo", "-cubin", "-DSIMLOD_RENDER_TIMERS=1", "-o", timed,
                     os.path.join(ROOT, "simlod_b200", "csrc", "render.cu")], capture_output=True, text=True)
 if r.returncode != 0:
     print("timers build failed:", r.stderr[-300:]); timed = None

@@ -25,7 +25,7 @@ if len(sys.argv) > 3 and sys.argv[3] != "-":
     import subprocess
     out = os.path.join(ROOT, "tools", "exp", "stress_variant.cubin")
     os.makedirs(os.path.dirname(out), exist_ok=True)
-    subprocess.check_call(["nvcc", "-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-std=c++17", "-lineinfo", "-cubin"] + sys.argv[3].split(",") + ["-o", out, os.path.join(ROOT, "simlod_b200", "csrc", "construct.cu")])
+    subprocess.check_call(["nvcc", "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-std=c++17", "-lineinfo", "-cubin"] + sys.argv[3].split(",") + ["-o", out, os.path.join(ROOT, "simlod_b200", "csrc", "construct.cu")])
     sim.use_module(0, out)
     print("variant", sys.argv[3], flush=True)
 for p in range(P):
