@@ -358,7 +358,8 @@ class SimLOD:
     def insert_batches(self, batches):
         """Insert explicit batches (each <= 1 M points), each followed by update launches until the
         device has consumed it (one batch per addBatch, as when the loader is slower than the GPU).
-        Returns the summed kernel ms."""
+        Returns the summed kernel ms. Raises SimlodError(SIMLOD_ERR_CAPACITY = -5) as soon as the builder refuses a batch
+        because the persistent heap is almost full, as simlod_insert* do."""
         total = 0.0
         done = self.stats().batchletIndex
         for b in batches:
@@ -367,7 +368,9 @@ class SimLOD:
             while True:
                 total += self.update_octree()
                 s = self.stats()
-                if s.batchletIndex >= done or s.memCapacityReached:
+                if s.memCapacityReached:
+                    raise SimlodError(-5, "persistent heap almost full after %d points" % s.numPointsProcessed)
+                if s.batchletIndex >= done:
                     break
         return total
 
