@@ -141,6 +141,29 @@ typedef struct SimlodHeapHeader {
     uint64_t offset;    // starts at 16; every alloc advances by 16*((size+16)/16)
 } SimlodHeapHeader;
 
+// One node of an exported octree (simlod_export_octree). Records are in breadth-first order: by level, then by the
+// Morton code of (X, Y, Z) with bit triples x<<2 | y<<1 | z (the child index), so the 8 children of a node are
+// consecutive records.
+enum {
+    SIMLOD_EXPORT_LEAF    = 1u << 0,   // the node has no children
+    SIMLOD_EXPORT_SAMPLED = 1u << 1,   // the node's samples are part of this export
+};
+typedef struct SimlodExportNode {
+    uint32_t level, X, Y, Z;           //  0  as in Node
+    uint8_t  name[20];                 // 16  as in Node
+    uint32_t flags;                    // 36  SIMLOD_EXPORT_*
+    int32_t  parent;                   // 40  record index, -1 for the root
+    int32_t  first_child;              // 44  record index of child 0, -1 if it has no children or they are not exported
+    uint64_t sample_offset;            // 48  index of its first sample in the sample array
+    uint32_t num_points;               // 56  exported points, stored first
+    uint32_t num_voxels;               // 60  exported voxels, stored right after the points
+} SimlodExportNode;
+
+typedef struct SimlodExportInfo {
+    uint32_t num_nodes, max_level;     // records in this export; deepest level in the octree
+    uint64_t num_samples, num_points, num_voxels;
+} SimlodExportInfo;
+
 SIMLOD_STATIC_ASSERT(sizeof(SimlodPoint) == 16, "Point");
 SIMLOD_STATIC_ASSERT(sizeof(SimlodChunk) == 16016, "Chunk");
 SIMLOD_STATIC_ASSERT(offsetof(SimlodChunk, size) == 16000, "Chunk.size");
@@ -181,3 +204,13 @@ SIMLOD_STATIC_ASSERT(offsetof(SimlodStats, numPointsProcessed) == 80, "Stats.num
 SIMLOD_STATIC_ASSERT(offsetof(SimlodStats, numAllocatedChunks) == 88, "Stats.numAllocatedChunks");
 SIMLOD_STATIC_ASSERT(offsetof(SimlodStats, chunkPoolSize) == 96, "Stats.chunkPoolSize");
 SIMLOD_STATIC_ASSERT(offsetof(SimlodStats, memCapacityReached) == 108, "Stats.memCapacityReached");
+SIMLOD_STATIC_ASSERT(sizeof(SimlodExportNode) == 64, "ExportNode");
+SIMLOD_STATIC_ASSERT(offsetof(SimlodExportNode, name) == 16, "ExportNode.name");
+SIMLOD_STATIC_ASSERT(offsetof(SimlodExportNode, flags) == 36, "ExportNode.flags");
+SIMLOD_STATIC_ASSERT(offsetof(SimlodExportNode, parent) == 40, "ExportNode.parent");
+SIMLOD_STATIC_ASSERT(offsetof(SimlodExportNode, first_child) == 44, "ExportNode.first_child");
+SIMLOD_STATIC_ASSERT(offsetof(SimlodExportNode, sample_offset) == 48, "ExportNode.sample_offset");
+SIMLOD_STATIC_ASSERT(offsetof(SimlodExportNode, num_points) == 56, "ExportNode.num_points");
+SIMLOD_STATIC_ASSERT(offsetof(SimlodExportNode, num_voxels) == 60, "ExportNode.num_voxels");
+SIMLOD_STATIC_ASSERT(sizeof(SimlodExportInfo) == 32, "ExportInfo");
+SIMLOD_STATIC_ASSERT(offsetof(SimlodExportInfo, num_samples) == 8, "ExportInfo.num_samples");

@@ -144,6 +144,22 @@ int simlod_read_framebuffer(SimlodContext* ctx, uint64_t* out);
 // RGBA8 surface written by kernel_render, width*height u32 (what the reference displays)
 int simlod_read_surface(SimlodContext* ctx, uint32_t* out);
 
+// Octree export: the node hierarchy and its samples as flat arrays in device memory, read from the ABI alone (Node
+// children, points / numPoints, voxelChunks / numVoxelsStored; up to 1000 samples per chunk, in chunk-list order), so it
+// works the same on an octree built by the reference kernels. A snapshot of the octree as the last completed
+// kernel_construct left it; it writes nothing into the context's buffers or Stats.
+//   depth < 0        every node, with its points and its voxels (SIMLOD_EXPORT_SAMPLED on every record)
+//   0 <= depth <= 20 records for the nodes of level <= depth; samples for the cut at `depth`: the voxels of each inner
+//                    node at level == depth and the points of each leaf at level <= depth (each region covered once)
+// dst_nodes receives SimlodExportNode records (node_capacity of them), dst_samples 16-byte SimlodPoint samples
+// (sample_capacity of them); both device addresses, 16-byte aligned. With dst_nodes == dst_samples == 0 only *info is
+// filled (size query). SIMLOD_ERR_INVALID, with nothing written to dst_*, for a capacity below *info's counts, depth > 20
+// or an inconsistent image (a child pointer outside nodes[], an inner node without 8 children, a chunk pointer outside
+// the used heap, a list shorter than its count). Enqueued on the launch stream; returns once the export has completed.
+// *kernel_ms (optional) = event time of the export kernels. Scratch memory is the context's, kept until simlod_destroy.
+int simlod_export_octree(SimlodContext* ctx, int32_t depth, uint64_t dst_nodes, uint64_t node_capacity,
+                         uint64_t dst_samples, uint64_t sample_capacity, SimlodExportInfo* info, float* kernel_ms);
+
 // Raw access for tests and tools: device addresses and sizes of the buffers the kernels share
 // (nodes[], persistent heap, momentary buffer, render buffer, point ring) and a bounded copy.
 typedef struct SimlodBuffers {

@@ -24,6 +24,11 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libsimlod_b200.so")
 
 POINT_DTYPE = np.dtype([("x", "<f4"), ("y", "<f4"), ("z", "<f4"), ("color", "<u4")])
+# SimlodExportNode (include/simlod_abi.h), 64 bytes
+EXPORT_NODE_DTYPE = np.dtype([
+    ("level", "<u4"), ("X", "<u4"), ("Y", "<u4"), ("Z", "<u4"), ("name", "S20"), ("flags", "<u4"),
+    ("parent", "<i4"), ("first_child", "<i4"), ("sample_offset", "<u8"), ("num_points", "<u4"), ("num_voxels", "<u4")])
+EXPORT_LEAF, EXPORT_SAMPLED = 1, 2
 
 MAX_BATCH_SIZE = 1_000_000
 BATCH_STREAM_SIZE = 50
@@ -105,7 +110,21 @@ class Buffers(C.Structure):
         "renderbuffer", "renderbuffer_bytes", "ring", "ring_bytes", "stats")]
 
 
+class ExportInfo(C.Structure):
+    """SimlodExportInfo: records in the export, deepest level in the octree, sample counts."""
+    _fields_ = [("num_nodes", C.c_uint32), ("max_level", C.c_uint32), ("num_samples", C.c_uint64), ("num_points", C.c_uint64),
+                ("num_voxels", C.c_uint64)]
+
+
+class OctreeExport:
+    """SimLOD.export_octree(): `nodes` (EXPORT_NODE_DTYPE records, breadth-first), `samples` (the sample array), `info`."""
+
+    def __init__(self, nodes, samples, info):
+        self.nodes, self.samples, self.info = nodes, samples, info
+
+
 assert C.sizeof(Uniforms) == 480 and C.sizeof(Stats) == 112
+assert C.sizeof(ExportInfo) == 32 and EXPORT_NODE_DTYPE.itemsize == 64
 
 # every symbol include/simlod_b200.h declares
 EXPORTS = [
@@ -117,6 +136,7 @@ EXPORTS = [
     "simlod_get_launch_info", "simlod_device_rcp", "simlod_synchronize", "simlod_flush_l2",
     "simlod_partition_count", "simlod_partition_scatter", "simlod_partition_wait",
     "simlod_export_framebuffer", "simlod_peer_signal", "simlod_composite_framebuffers", "simlod_generate", "simlod_reset_with_grid", "simlod_insert_simlod_file_ex", "simlod_get_numa_node",
+    "simlod_export_octree",
 ]
 
 _lib = None
@@ -172,6 +192,7 @@ def load_library():
         "simlod_export_framebuffer": [vp, u64],
         "simlod_peer_signal": [vp, C.POINTER(u64), u32, u32],
         "simlod_composite_framebuffers": [vp, C.POINTER(u64), u32, u32, C.POINTER(u64), u32],
+        "simlod_export_octree": [vp, C.c_int32, u64, u64, u64, u64, C.POINTER(ExportInfo), C.POINTER(C.c_float)],
     }
     for name, argtypes in sig.items():
         fn = getattr(lib, name)
@@ -417,6 +438,48 @@ class SimLOD:
         heap_used = int(self.memcpy_dtoh(b.persistent + 8, 8).view(np.uint64)[0])
         heap = self.memcpy_dtoh(b.persistent, heap_used)
         return nodes, heap, int(b.nodes), int(b.persistent)
+
+    def export_octree_into(self, depth, dst_nodes, node_capacity, dst_samples, sample_capacity):
+        """simlod_export_octree into caller-owned device memory (depth None or < 0: full export; all zero: size query).
+        Returns (ExportInfo, kernel ms)."""
+        info, ms = ExportInfo(), C.c_float(0)
+        d = -1 if depth is None else int(depth)
+        self._check(self._lib.simlod_export_octree(self._ctx, d, int(dst_nodes), int(node_capacity), int(dst_samples),
+                                                   int(sample_capacity), C.byref(info), C.byref(ms)))
+        return info, ms.value
+
+    def export_octree(self, depth=None, device="cuda"):
+        """The octree as flat arrays (simlod_export_octree): depth=None exports every node with its points and voxels, an
+        integer depth the cut at that level (the voxels of the inner nodes at `depth`, the points of the leaves above).
+        Returns an OctreeExport: `nodes` (numpy EXPORT_NODE_DTYPE), `samples` and `info` (ExportInfo). With device="cuda"
+        the samples stay in device memory as a float32 torch tensor of shape (N, 4) (x, y, z, colour bits:
+        `.view(torch.int32)[:, 3]` is the colour); with device="cpu" they are a numpy POINT_DTYPE array."""
+        info, _ = self.export_octree_into(depth, 0, 0, 0, 0)
+        n, m = info.num_nodes, info.num_samples
+        if device == "cpu":
+            dn = self.device_alloc(n * 64)
+            ds = self.device_alloc(m * 16) if m else 0
+            try:
+                info, _ = self.export_octree_into(depth, dn, n, ds, m)
+                nodes = self.memcpy_dtoh(dn, n * 64).view(EXPORT_NODE_DTYPE)
+                samples = self.memcpy_dtoh(ds, m * 16).view(POINT_DTYPE)
+            finally:
+                self.device_free(dn)
+                if ds:
+                    self.device_free(ds)
+            return OctreeExport(nodes, samples, info)
+        import torch
+        dev = torch.device(device)
+        if dev.type != "cuda":
+            raise ValueError("device must be 'cpu' or a CUDA device, not %r" % device)
+        if dev.index is None:
+            dev = torch.device("cuda", self.device)
+        nodes_t = torch.empty(n * 64, dtype=torch.uint8, device=dev)
+        samples = torch.empty((m, 4), dtype=torch.float32, device=dev)
+        torch.cuda.current_stream(dev).synchronize()       # the caching allocator may hand out memory torch still uses
+        info, _ = self.export_octree_into(depth, nodes_t.data_ptr(), n, samples.data_ptr() if m else 0, m)
+        nodes = nodes_t.cpu().numpy().view(EXPORT_NODE_DTYPE)
+        return OctreeExport(nodes, samples, info)
 
     def host_alloc(self, nbytes):
         p = C.c_void_p()

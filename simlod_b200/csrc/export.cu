@@ -1,0 +1,249 @@
+// export.cu — octree export: the node hierarchy and its samples as flat arrays (DESIGN.md §9.4).
+//
+// Reads the ABI only (Node::children, points / numPoints, voxelChunks / numVoxelsStored, the heap header and
+// Stats::numNodes), so an octree built by the reference kernels exports exactly like ours. Three launches:
+//
+//   simlod_export_plan     one block: breadth-first order level by level from the root (records in (level, Morton) order,
+//                          the 8 children of a node consecutive), per-record sample counts, the exclusive scans that give
+//                          sample_offset and each list's first chunk item, and ExportCtl (sizes + error)
+//   simlod_export_collect  one thread per sampled record walks its chunk lists (the dependent ->next chains), tests every
+//                          pointer before it dereferences it and writes one item per chunk: source chunk, destination
+//                          index, count
+//   simlod_export_gather   after the host has checked ExportCtl: warps copy the node records, then pop chunk items
+//                          (<= 1000 samples each) and copy them with 16-byte loads and coalesced streaming stores
+//
+// The plan and collect kernels write scratch and ExportCtl only; nothing reaches the destination before the gather.
+#include <stdint.h>
+#include "../../include/simlod_abi.h"
+
+constexpr uint32_t PLAN_THREADS = 1024;
+constexpr uint32_t PPC = SIMLOD_POINTS_PER_CHUNK;
+
+enum : uint32_t {                         // ExportCtl::error (the canonicaliser's codes, oracle.cpp canonFromImage)
+    EXPORT_ERR_CHILD = 1,                 // a child pointer outside nodes[] (or more records than nodes: a node reached twice)
+    EXPORT_ERR_CHUNK = 2,                 // a chunk pointer outside the used heap
+    EXPORT_ERR_SHORT = 4,                 // a list shorter than its count
+    EXPORT_ERR_PARTIAL = 5,               // an inner node without all 8 children
+};
+
+struct ExportCtl {                        // mirrors host.cpp
+    uint32_t numNodes, maxLevel;
+    uint64_t numSamples, numPoints, numVoxels;
+    uint64_t numItems;
+    uint32_t error, pad;
+};
+
+struct Item { uint64_t src; uint64_t dst; };   // dst: sample index | count << 48
+
+__device__ __forceinline__ uint32_t ceilChunks(uint32_t n) { return (n + PPC - 1) / PPC; }
+
+// Block-wide exclusive scan (PLAN_THREADS threads) of 64-bit values; returns the prefix, *total the sum.
+__device__ uint64_t blockScan(uint64_t v, uint64_t* total) {
+    __shared__ uint64_t warpSums[PLAN_THREADS / 32];
+    const uint32_t lane = threadIdx.x & 31u, warp = threadIdx.x >> 5;
+    uint64_t x = v;
+    for (uint32_t o = 1; o < 32; o <<= 1) {
+        uint64_t y = __shfl_up_sync(0xffffffffu, x, o);
+        if (lane >= o) x += y;
+    }
+    if (lane == 31) warpSums[warp] = x;
+    __syncthreads();
+    if (warp == 0) {
+        uint64_t s = warpSums[lane];
+        for (uint32_t o = 1; o < 32; o <<= 1) {
+            uint64_t y = __shfl_up_sync(0xffffffffu, s, o);
+            if (lane >= o) s += y;
+        }
+        warpSums[lane] = s;
+    }
+    __syncthreads();
+    const uint64_t prefix = (warp ? warpSums[warp - 1] : 0) + x - v;
+    *total = warpSums[PLAN_THREADS / 32 - 1];
+    __syncthreads();                       // warpSums is reused by the next call
+    return prefix;
+}
+
+// depth < 0: full export. Scratch: rec[maxRecords] (SimlodExportNode), recNode[maxRecords] (node index),
+// recItem[maxRecords] (first chunk item of the record's point list; its voxel list follows).
+extern "C" __global__ void __launch_bounds__(PLAN_THREADS)
+simlod_export_plan(const uint8_t* __restrict__ nodes, const SimlodStats* __restrict__ stats, int32_t depth, uint32_t maxRecords,
+                   SimlodExportNode* __restrict__ rec, uint32_t* __restrict__ recNode, uint64_t* __restrict__ recItem,
+                   ExportCtl* __restrict__ ctl) {
+    __shared__ uint32_t sh_total, sh_error, sh_maxLevel;
+    const uint32_t numNodes = stats->numNodes;
+    const uint64_t nodesAddr = (uint64_t)nodes;
+    if (threadIdx.x == 0) {
+        sh_total = 1; sh_error = 0; sh_maxLevel = 0;
+        if (numNodes == 0 || numNodes > maxRecords) sh_error = EXPORT_ERR_CHILD;
+        recNode[0] = 0;
+        rec[0].parent = -1;
+    }
+    __syncthreads();
+    if (sh_error) { if (threadIdx.x == 0) ctl->error = sh_error; return; }
+
+    // deepest level in the octree: every allocated node
+    uint32_t lmax = 0;
+    for (uint32_t i = threadIdx.x; i < numNodes; i += PLAN_THREADS)
+        lmax = max(lmax, ((const SimlodNode*)(nodes + (uint64_t)i * sizeof(SimlodNode)))->level);
+    atomicMax(&sh_maxLevel, lmax);
+
+    // breadth-first, level by level: the children of the records [begin, end) are appended in record order, 8 per inner
+    // node in child-index order, which is (level, Morton) order one level down
+    uint32_t begin = 0, end = 1;
+    for (int32_t level = 0; begin < end; level++) {
+        const bool expand = depth < 0 || level < depth;
+        for (uint32_t tile = begin; tile < end; tile += PLAN_THREADS) {
+            const uint32_t r = tile + threadIdx.x;
+            const bool valid = r < end;
+            uint32_t numChildren = 0, err = 0;
+            uint64_t child[8];
+            const SimlodNode* node = nullptr;
+            if (valid) {
+                node = (const SimlodNode*)(nodes + (uint64_t)recNode[r] * sizeof(SimlodNode));
+                #pragma unroll
+                for (int k = 0; k < 8; k++) {
+                    child[k] = (uint64_t)node->children[k];
+                    if (child[k]) {
+                        numChildren++;
+                        const uint64_t off = child[k] - nodesAddr;
+                        if (child[k] < nodesAddr || off % sizeof(SimlodNode) != 0 || off / sizeof(SimlodNode) >= numNodes) err = EXPORT_ERR_CHILD;
+                    }
+                }
+                if (numChildren != 0 && numChildren != 8) err = EXPORT_ERR_PARTIAL;
+            }
+            const bool inner = numChildren == 8;
+            uint64_t total = 0;
+            const uint32_t pos = (uint32_t)blockScan(valid && expand && inner && !err ? 8 : 0, &total);
+            const uint32_t first = sh_total + pos;
+            __syncthreads();
+            if (threadIdx.x == 0) {
+                if (sh_total + total > numNodes) atomicMax(&sh_error, EXPORT_ERR_CHILD);   // more records than nodes
+                else sh_total += (uint32_t)total;
+            }
+            if (err) atomicMax(&sh_error, err);
+            if (valid) {
+                const bool addChildren = expand && inner && !err && first + 8 <= numNodes;
+                if (addChildren) {
+                    #pragma unroll
+                    for (int k = 0; k < 8; k++) {
+                        recNode[first + k] = (uint32_t)((child[k] - nodesAddr) / sizeof(SimlodNode));
+                        rec[first + k].parent = (int32_t)r;
+                    }
+                }
+                // what this record contributes: everything (full), the voxels of an inner node at the cut level, the
+                // points of a leaf at or above it
+                const uint32_t np = node->numPoints, nv = node->numVoxelsStored;
+                const bool full = depth < 0;
+                const bool sampled = full || !inner || level == depth;
+                SimlodExportNode& o = rec[r];
+                o.level = node->level; o.X = node->X; o.Y = node->Y; o.Z = node->Z;
+                const uint32_t* nm = (const uint32_t*)node->name;
+                uint32_t* onm = (uint32_t*)o.name;
+                #pragma unroll
+                for (int k = 0; k < 5; k++) onm[k] = nm[k];
+                o.flags = (inner ? 0u : (uint32_t)SIMLOD_EXPORT_LEAF) | (sampled ? (uint32_t)SIMLOD_EXPORT_SAMPLED : 0u);
+                o.first_child = addChildren ? (int32_t)first : -1;
+                o.num_points = full || !inner ? np : 0;
+                o.num_voxels = full || (inner && level == depth) ? nv : 0;
+            }
+            __syncthreads();
+            if (sh_error) break;
+        }
+        if (sh_error) break;
+        begin = end;
+        end = sh_total;
+    }
+    __syncthreads();
+    if (sh_error) { if (threadIdx.x == 0) ctl->error = sh_error; return; }
+
+    // sample offsets and chunk items: exclusive scans over the records
+    const uint32_t n = sh_total;
+    uint64_t samplesBase = 0, itemsBase = 0, points = 0, voxels = 0;
+    for (uint32_t tile = 0; tile < n; tile += PLAN_THREADS) {
+        const uint32_t r = tile + threadIdx.x;
+        uint32_t np = 0, nv = 0;
+        if (r < n) { np = rec[r].num_points; nv = rec[r].num_voxels; }
+        uint64_t tS = 0, tI = 0, tP = 0, tV = 0;
+        const uint64_t s = blockScan((uint64_t)np + nv, &tS);
+        const uint64_t it = blockScan(ceilChunks(np) + ceilChunks(nv), &tI);
+        blockScan(np, &tP);
+        blockScan(nv, &tV);
+        if (r < n) { rec[r].sample_offset = samplesBase + s; recItem[r] = itemsBase + it; }
+        samplesBase += tS; itemsBase += tI; points += tP; voxels += tV;
+    }
+    if (threadIdx.x == 0) {
+        ctl->numNodes = n; ctl->maxLevel = sh_maxLevel;
+        ctl->numSamples = samplesBase; ctl->numPoints = points; ctl->numVoxels = voxels;
+        ctl->numItems = itemsBase; ctl->error = 0;
+    }
+}
+
+// Walks `count` samples' worth of chunks of the list at `head`. Every chunk must lie inside the used heap
+// [heap, heap + heapUsed) and be 16-byte aligned before it is read; the list must not end early.
+__device__ __forceinline__ uint32_t walkList(uint64_t head, uint32_t count, uint64_t heap, uint64_t heapUsed, uint64_t dst,
+                                             Item* __restrict__ items) {
+    uint64_t addr = head;
+    for (uint32_t c = 0; c < ceilChunks(count); c++) {
+        if (addr == 0) return EXPORT_ERR_SHORT;
+        if (addr < heap || addr - heap > heapUsed || heapUsed - (addr - heap) < sizeof(SimlodChunk) || (addr - heap) % 16 != 0)
+            return EXPORT_ERR_CHUNK;
+        const uint32_t take = min(count - c * PPC, PPC);
+        items[c] = Item{addr, (dst + (uint64_t)c * PPC) | ((uint64_t)take << 48)};
+        addr = (uint64_t)((const SimlodChunk*)addr)->next;
+    }
+    return 0;
+}
+
+extern "C" __global__ void __launch_bounds__(256)
+simlod_export_collect(const uint8_t* __restrict__ nodes, const uint8_t* __restrict__ heap, uint64_t heapBytes,
+                      const SimlodExportNode* __restrict__ rec, const uint32_t* __restrict__ recNode, const uint64_t* __restrict__ recItem,
+                      Item* __restrict__ items, uint64_t itemsCap, ExportCtl* __restrict__ ctl) {
+    if (ctl->error) return;
+    // more chunks than the used heap can hold: the counts do not match the lists (the scratch holds one item per chunk)
+    if (ctl->numItems > itemsCap) { if (blockIdx.x == 0 && threadIdx.x == 0) atomicMax(&ctl->error, (uint32_t)EXPORT_ERR_SHORT); return; }
+    const uint32_t n = ctl->numNodes;
+    const uint64_t heapAddr = (uint64_t)heap;
+    const uint64_t heapUsed = min(((const SimlodHeapHeader*)heap)->offset, heapBytes);
+    for (uint32_t r = blockIdx.x * blockDim.x + threadIdx.x; r < n; r += gridDim.x * blockDim.x) {
+        const uint32_t np = rec[r].num_points, nv = rec[r].num_voxels;
+        if (np == 0 && nv == 0) continue;
+        const SimlodNode* node = (const SimlodNode*)(nodes + (uint64_t)recNode[r] * sizeof(SimlodNode));
+        const uint64_t base = recItem[r], dst = rec[r].sample_offset;
+        uint32_t err = walkList((uint64_t)node->points, np, heapAddr, heapUsed, dst, items + base);
+        if (!err) err = walkList((uint64_t)node->voxelChunks, nv, heapAddr, heapUsed, dst + np, items + base + ceilChunks(np));
+        if (err) atomicMax(&ctl->error, err);
+    }
+}
+
+constexpr uint32_t GATHER_UNROLL = 8;
+
+extern "C" __global__ void __launch_bounds__(256)
+simlod_export_gather(const uint4* __restrict__ rec, uint4* __restrict__ dstNodes, const Item* __restrict__ items,
+                     uint4* __restrict__ dstSamples, const ExportCtl* __restrict__ ctl) {
+    const uint32_t lane = threadIdx.x & 31u;
+    const uint64_t warp = ((uint64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    const uint64_t numWarps = ((uint64_t)gridDim.x * blockDim.x) >> 5;
+    const uint64_t recWords = (uint64_t)ctl->numNodes * (sizeof(SimlodExportNode) / 16);
+    for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < recWords; i += (uint64_t)gridDim.x * blockDim.x)
+        __stcs(dstNodes + i, rec[i]);
+    const uint64_t numItems = ctl->numItems;
+    for (uint64_t k = warp; k < numItems; k += numWarps) {
+        const Item it = items[k];
+        const uint4* __restrict__ src = (const uint4*)it.src;
+        uint4* __restrict__ dst = dstSamples + (it.dst & 0xffffffffffffull);
+        const uint32_t count = (uint32_t)(it.dst >> 48);
+        for (uint32_t b = 0; b < count; b += 32 * GATHER_UNROLL) {
+            uint4 v[GATHER_UNROLL];
+            #pragma unroll
+            for (uint32_t u = 0; u < GATHER_UNROLL; u++) {
+                const uint32_t j = b + u * 32 + lane;
+                if (j < count) v[u] = __ldcs(src + j);
+            }
+            #pragma unroll
+            for (uint32_t u = 0; u < GATHER_UNROLL; u++) {
+                const uint32_t j = b + u * 32 + lane;
+                if (j < count) __stcs(dst + j, v[u]);
+            }
+        }
+    }
+}

@@ -42,6 +42,7 @@ extern const unsigned char simlod_cubin_util[];
 extern const unsigned char simlod_cubin_partition[];
 extern const unsigned char simlod_cubin_las[];
 extern const unsigned char simlod_cubin_gen[];
+extern const unsigned char simlod_cubin_export[];
 }
 
 namespace {
@@ -152,6 +153,11 @@ struct SimlodContext {
     uint32_t partNextSlot = 0;
     CUfunction fnLas = nullptr;
     CUdeviceptr lasStaging = 0;        // raw LAS records of the batch being decoded
+    CUmodule exportModule = nullptr;
+    CUfunction fnExportPlan = nullptr, fnExportCollect = nullptr, fnExportGather = nullptr;
+    CUdeviceptr exportScratch = 0;     // octree export: records | node indices | first items | chunk items | ExportCtl
+    uint64_t exportScratchBytes = 0;
+    void* hExportCtl = nullptr;        // pinned copy of ExportCtl
     void* pinnedPool = nullptr;        // POOL_SLOTS x 16 MB page-locked staging slots of the file streamer
     LoaderPool* loaderPool = nullptr;
     CUevent evPool[32] = {};           // H2D copy out of pool slot i has been enqueued and completed
@@ -432,6 +438,10 @@ static int createResources(SimlodContext* ctx, const SimlodConfig* config) {
     CU(D(cuModuleGetFunction)(&ctx->fnPartWait, ctx->partitionModule, "simlod_partition_wait"));
     CU(D(cuModuleGetFunction)(&ctx->fnComposite, ctx->partitionModule, "simlod_composite_min"));
     CU(D(cuModuleGetFunction)(&ctx->fnPeerSignal, ctx->partitionModule, "simlod_peer_signal"));
+    CU(D(cuModuleLoadData)(&ctx->exportModule, simlod_cubin_export));
+    CU(D(cuModuleGetFunction)(&ctx->fnExportPlan, ctx->exportModule, "simlod_export_plan"));
+    CU(D(cuModuleGetFunction)(&ctx->fnExportCollect, ctx->exportModule, "simlod_export_collect"));
+    CU(D(cuModuleGetFunction)(&ctx->fnExportGather, ctx->exportModule, "simlod_export_gather"));
 
     // buffers (main.cpp:552-586)
     SimlodBuffers& b = ctx->buf;
@@ -535,6 +545,9 @@ void simlod_destroy(SimlodContext* ctx) {
         if (ctx->lasModule) D(cuModuleUnload)(ctx->lasModule);
         if (ctx->genModule) D(cuModuleUnload)(ctx->genModule);
         if (ctx->lasStaging) D(cuMemFree)(ctx->lasStaging);
+        if (ctx->exportModule) D(cuModuleUnload)(ctx->exportModule);
+        if (ctx->exportScratch) D(cuMemFree)(ctx->exportScratch);
+        if (ctx->hExportCtl) D(cuMemFreeHost)(ctx->hExportCtl);
         delete ctx->loaderPool;          // joins the loader threads
         if (ctx->pinnedPool) D(cuMemFreeHost)(ctx->pinnedPool);
         for (int i = 0; i < 32; i++) if (ctx->evPool[i]) D(cuEventDestroy)(ctx->evPool[i]);
@@ -1108,6 +1121,77 @@ int simlod_flush_l2(SimlodContext* ctx) {
     CU(D(cuLaunchKernel)(ctx->fnFill, (unsigned)(ctx->numSMs * 8), 1, 1, 256, 1, 1, 0, ctx->streamMain, args, nullptr));
     ctx->launches++;
     CU(D(cuStreamSynchronize)(ctx->streamMain));
+    return SIMLOD_OK;
+}
+
+// ---- octree export (DESIGN.md §9.4); kernels in export.cu -------------------------------------------------
+namespace {
+struct ExportCtl {                   // mirrors export.cu
+    uint32_t numNodes, maxLevel;
+    uint64_t numSamples, numPoints, numVoxels;
+    uint64_t numItems;
+    uint32_t error, pad;
+};
+constexpr uint64_t align16(uint64_t v) { return (v + 15) & ~15ull; }
+}  // namespace
+
+int simlod_export_octree(SimlodContext* ctx, int32_t depth, uint64_t dst_nodes, uint64_t node_capacity,
+                         uint64_t dst_samples, uint64_t sample_capacity, SimlodExportInfo* info, float* kernel_ms) {
+    int rc = setCurrent(ctx); if (rc) return rc;
+    if (!info) return fail(SIMLOD_ERR_INVALID, "null info");
+    if (depth > SIMLOD_MAX_DEPTH) return fail(SIMLOD_ERR_INVALID, "export depth %d exceeds the octree's maximum depth %d", depth, (int)SIMLOD_MAX_DEPTH);
+    if (dst_nodes % 16 || dst_samples % 16) return fail(SIMLOD_ERR_INVALID, "export destinations must be 16-byte aligned");
+    // scratch, sized by the context's buffers: one record per node of nodes[], one item per chunk the heap can hold
+    const uint32_t maxRecords = (uint32_t)(ctx->buf.nodes_bytes / sizeof(SimlodNode));
+    const uint64_t itemsCap = ctx->buf.persistent_bytes / SIMLOD_CHUNK_STRIDE + 1;
+    const uint64_t offNode = align16((uint64_t)maxRecords * sizeof(SimlodExportNode)), offItem = offNode + align16((uint64_t)maxRecords * 4),
+                   offItems = offItem + align16((uint64_t)maxRecords * 8), offCtl = offItems + itemsCap * 16, bytes = offCtl + sizeof(ExportCtl);
+    if (ctx->exportScratchBytes < bytes) {
+        if (ctx->exportScratch) CU(D(cuMemFree)(ctx->exportScratch));
+        ctx->exportScratch = 0;
+        ctx->exportScratchBytes = 0;
+        CU(D(cuMemAlloc)(&ctx->exportScratch, bytes));
+        ctx->exportScratchBytes = bytes;
+    }
+    if (!ctx->hExportCtl) CU(D(cuMemHostAlloc)(&ctx->hExportCtl, sizeof(ExportCtl), 0));
+    CUdeviceptr nodes = ctx->buf.nodes, heap = ctx->buf.persistent, stats = ctx->buf.stats;
+    CUdeviceptr rec = ctx->exportScratch, recNode = rec + offNode, recItem = rec + offItem, items = rec + offItems, ctl = rec + offCtl;
+    uint64_t heapBytes = ctx->buf.persistent_bytes;
+    // stage 1: plan (one block) and the chunk-list walk, both into scratch only
+    CU(D(cuEventRecord)(ctx->evStart, ctx->streamMain));
+    { void* args[] = {&nodes, &stats, &depth, (void*)&maxRecords, &rec, &recNode, &recItem, &ctl};
+      CU(D(cuLaunchKernel)(ctx->fnExportPlan, 1, 1, 1, 1024, 1, 1, 0, ctx->streamMain, args, nullptr)); }
+    uint64_t cap = itemsCap;
+    { void* args[] = {&nodes, &heap, &heapBytes, &rec, &recNode, &recItem, &items, &cap, &ctl};
+      CU(D(cuLaunchKernel)(ctx->fnExportCollect, (unsigned)ctx->numSMs * 2, 1, 1, 256, 1, 1, 0, ctx->streamMain, args, nullptr)); }
+    CU(D(cuEventRecord)(ctx->evEnd, ctx->streamMain));
+    ctx->launches += 2;
+    CU(D(cuMemcpyDtoHAsync)(ctx->hExportCtl, ctl, sizeof(ExportCtl), ctx->streamMain));
+    CU(D(cuStreamSynchronize)(ctx->streamMain));
+    const ExportCtl c = *(const ExportCtl*)ctx->hExportCtl;
+    float ms = 0.0f;
+    CU(D(cuEventElapsedTime)(&ms, ctx->evStart, ctx->evEnd));
+    if (kernel_ms) *kernel_ms = ms;
+    if (c.error)
+        return fail(SIMLOD_ERR_INVALID, "octree image is inconsistent (error %u: 1 child pointer outside nodes[], 2 chunk pointer outside the used heap, 4 list shorter than its count, 5 inner node without 8 children)", c.error);
+    info->num_nodes = c.numNodes; info->max_level = c.maxLevel;
+    info->num_samples = c.numSamples; info->num_points = c.numPoints; info->num_voxels = c.numVoxels;
+    if (!dst_nodes && !dst_samples) return SIMLOD_OK;          // size query
+    if (!dst_nodes || node_capacity < c.numNodes)
+        return fail(SIMLOD_ERR_INVALID, "node destination holds %llu records, the export has %u", (unsigned long long)(dst_nodes ? node_capacity : 0), c.numNodes);
+    if (c.numSamples && (!dst_samples || sample_capacity < c.numSamples))
+        return fail(SIMLOD_ERR_INVALID, "sample destination holds %llu samples, the export has %llu", (unsigned long long)(dst_samples ? sample_capacity : 0), (unsigned long long)c.numSamples);
+    // stage 2: gather into the destination
+    CUdeviceptr dn = (CUdeviceptr)dst_nodes, ds = (CUdeviceptr)dst_samples;
+    CU(D(cuEventRecord)(ctx->evTotalStart, ctx->streamMain));
+    { void* args[] = {&rec, &dn, &items, &ds, &ctl};
+      CU(D(cuLaunchKernel)(ctx->fnExportGather, (unsigned)ctx->numSMs * 4, 1, 1, 256, 1, 1, 0, ctx->streamMain, args, nullptr)); }
+    CU(D(cuEventRecord)(ctx->evTotalEnd, ctx->streamMain));
+    ctx->launches++;
+    CU(D(cuEventSynchronize)(ctx->evTotalEnd));
+    float gatherMs = 0.0f;
+    CU(D(cuEventElapsedTime)(&gatherMs, ctx->evTotalStart, ctx->evTotalEnd));
+    if (kernel_ms) *kernel_ms = ms + gatherMs;
     return SIMLOD_OK;
 }
 
