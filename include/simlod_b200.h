@@ -160,6 +160,18 @@ int simlod_read_surface(SimlodContext* ctx, uint32_t* out);
 int simlod_export_octree(SimlodContext* ctx, int32_t depth, uint64_t dst_nodes, uint64_t node_capacity,
                          uint64_t dst_samples, uint64_t sample_capacity, SimlodExportInfo* info, float* kernel_ms);
 
+// View export: the LOD cut simlod_render draws for the current uniforms (transform_updateBound, so a frozen visibility
+// transform is honoured; width, height, minNodeSize, the box), in the records and samples of simlod_export_octree. A node
+// is drawn when it is visible and either a large leaf, or not large with a large parent, evaluated per node of
+// nodes[0, Stats::numNodes) by the renderer's own arithmetic. Records: the root and the 8 children of every inner node
+// with a drawn node strictly below it, breadth-first; SIMLOD_EXPORT_SAMPLED exactly on the drawn nodes, which carry their
+// points and their stored voxels; the others carry none. Nothing drawn: the root record alone. Render-time colouring does
+// not apply. Destinations, size query, errors and scratch as for simlod_export_octree; a drawn node the breadth-first
+// pass does not reach is reported as a child pointer error. Unlike simlod_render it writes nothing into nodes[] (not
+// even the visible / isLarge flags) or any other buffer of the context.
+int simlod_export_view(SimlodContext* ctx, uint64_t dst_nodes, uint64_t node_capacity, uint64_t dst_samples,
+                       uint64_t sample_capacity, SimlodExportInfo* info, float* kernel_ms);
+
 // Raw access for tests and tools: device addresses and sizes of the buffers the kernels share
 // (nodes[], persistent heap, momentary buffer, render buffer, point ring) and a bounded copy.
 typedef struct SimlodBuffers {

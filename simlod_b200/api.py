@@ -117,7 +117,8 @@ class ExportInfo(C.Structure):
 
 
 class OctreeExport:
-    """SimLOD.export_octree(): `nodes` (EXPORT_NODE_DTYPE records, breadth-first), `samples` (the sample array), `info`."""
+    """SimLOD.export_octree() / export_view(): `nodes` (EXPORT_NODE_DTYPE records, breadth-first), `samples` (the sample
+    array), `info`."""
 
     def __init__(self, nodes, samples, info):
         self.nodes, self.samples, self.info = nodes, samples, info
@@ -136,7 +137,7 @@ EXPORTS = [
     "simlod_get_launch_info", "simlod_device_rcp", "simlod_synchronize", "simlod_flush_l2",
     "simlod_partition_count", "simlod_partition_scatter", "simlod_partition_wait",
     "simlod_export_framebuffer", "simlod_peer_signal", "simlod_composite_framebuffers", "simlod_generate", "simlod_reset_with_grid", "simlod_insert_simlod_file_ex", "simlod_get_numa_node",
-    "simlod_export_octree",
+    "simlod_export_octree", "simlod_export_view",
 ]
 
 _lib = None
@@ -193,6 +194,7 @@ def load_library():
         "simlod_peer_signal": [vp, C.POINTER(u64), u32, u32],
         "simlod_composite_framebuffers": [vp, C.POINTER(u64), u32, u32, C.POINTER(u64), u32],
         "simlod_export_octree": [vp, C.c_int32, u64, u64, u64, u64, C.POINTER(ExportInfo), C.POINTER(C.c_float)],
+        "simlod_export_view": [vp, u64, u64, u64, u64, C.POINTER(ExportInfo), C.POINTER(C.c_float)],
     }
     for name, argtypes in sig.items():
         fn = getattr(lib, name)
@@ -454,13 +456,31 @@ class SimLOD:
         Returns an OctreeExport: `nodes` (numpy EXPORT_NODE_DTYPE), `samples` and `info` (ExportInfo). With device="cuda"
         the samples stay in device memory as a float32 torch tensor of shape (N, 4) (x, y, z, colour bits:
         `.view(torch.int32)[:, 3]` is the colour); with device="cpu" they are a numpy POINT_DTYPE array."""
-        info, _ = self.export_octree_into(depth, 0, 0, 0, 0)
+        return self._export(lambda *dst: self.export_octree_into(depth, *dst), device)
+
+    def export_view_into(self, dst_nodes, node_capacity, dst_samples, sample_capacity):
+        """simlod_export_view into caller-owned device memory (all zero: size query). Returns (ExportInfo, kernel ms)."""
+        info, ms = ExportInfo(), C.c_float(0)
+        self._check(self._lib.simlod_export_view(self._ctx, int(dst_nodes), int(node_capacity), int(dst_samples),
+                                                 int(sample_capacity), C.byref(info), C.byref(ms)))
+        return info, ms.value
+
+    def export_view(self, device="cuda"):
+        """The LOD cut render() draws for the current camera and settings, as flat arrays (simlod_export_view): the drawn
+        nodes flagged EXPORT_SAMPLED with their points and voxels, and the records that link them to the root. Writes no
+        visibility flags. Returns an OctreeExport, with `samples` on `device` as for export_octree."""
+        return self._export(self.export_view_into, device)
+
+    def _export(self, into, device):
+        """Size query, then the export into arrays of that size: into(dst_nodes, node_capacity, dst_samples,
+        sample_capacity) -> (ExportInfo, ms)."""
+        info, _ = into(0, 0, 0, 0)
         n, m = info.num_nodes, info.num_samples
         if device == "cpu":
             dn = self.device_alloc(n * 64)
             ds = self.device_alloc(m * 16) if m else 0
             try:
-                info, _ = self.export_octree_into(depth, dn, n, ds, m)
+                info, _ = into(dn, n, ds, m)
                 nodes = self.memcpy_dtoh(dn, n * 64).view(EXPORT_NODE_DTYPE)
                 samples = self.memcpy_dtoh(ds, m * 16).view(POINT_DTYPE)
             finally:
@@ -477,7 +497,7 @@ class SimLOD:
         nodes_t = torch.empty(n * 64, dtype=torch.uint8, device=dev)
         samples = torch.empty((m, 4), dtype=torch.float32, device=dev)
         torch.cuda.current_stream(dev).synchronize()       # the caching allocator may hand out memory torch still uses
-        info, _ = self.export_octree_into(depth, nodes_t.data_ptr(), n, samples.data_ptr() if m else 0, m)
+        info, _ = into(nodes_t.data_ptr(), n, samples.data_ptr() if m else 0, m)
         nodes = nodes_t.cpu().numpy().view(EXPORT_NODE_DTYPE)
         return OctreeExport(nodes, samples, info)
 

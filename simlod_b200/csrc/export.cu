@@ -1,20 +1,28 @@
-// export.cu — octree export: the node hierarchy and its samples as flat arrays (DESIGN.md §9.4).
+// export.cu — octree export: the node hierarchy and its samples as flat arrays (DESIGN.md §9.4), whole, cut at one
+// depth, or the LOD cut one camera sees (§9.5).
 //
 // Reads the ABI only (Node::children, points / numPoints, voxelChunks / numVoxelsStored, the heap header and
-// Stats::numNodes), so an octree built by the reference kernels exports exactly like ours. Three launches:
+// Stats::numNodes; for the view also the fields the renderer's cut reads), so an octree built by the reference kernels
+// exports exactly like ours. Three launches, four for the view:
 //
+//   simlod_export_view_flags  (view only) one thread per node of nodes[]: whether kernel_render would draw it for the
+//                          uniforms, by the renderer's own test (nodeDrawn, lodcut.cuh), as one byte per node index
 //   simlod_export_plan     one block: breadth-first order level by level from the root (records in (level, Morton) order,
 //                          the 8 children of a node consecutive), per-record sample counts, the exclusive scans that give
-//                          sample_offset and each list's first chunk item, and ExportCtl (sizes + error)
+//                          sample_offset and each list's first chunk item, and ExportCtl (sizes + error);
+//                          simlod_export_plan_view, the view's instance of the same code, cuts the breadth-first records
+//                          down to the paths that reach the drawn nodes
 //   simlod_export_collect  one thread per sampled record walks its chunk lists (the dependent ->next chains), tests every
 //                          pointer before it dereferences it and writes one item per chunk: source chunk, destination
 //                          index, count
 //   simlod_export_gather   after the host has checked ExportCtl: warps copy the node records, then pop chunk items
 //                          (<= 1000 samples each) and copy them with 16-byte loads and coalesced streaming stores
 //
-// The plan and collect kernels write scratch and ExportCtl only; nothing reaches the destination before the gather.
+// The flags, plan and collect kernels write scratch and ExportCtl only; nothing reaches the destination before the
+// gather. Nothing is written into nodes[] (not even the visible / isLarge flags kernel_render stores there).
 #include <stdint.h>
 #include "../../include/simlod_abi.h"
+#include "lodcut.cuh"
 
 constexpr uint32_t PLAN_THREADS = 1024;
 constexpr uint32_t PPC = SIMLOD_POINTS_PER_CHUNK;
@@ -37,7 +45,9 @@ struct Item { uint64_t src; uint64_t dst; };   // dst: sample index | count << 4
 
 __device__ __forceinline__ uint32_t ceilChunks(uint32_t n) { return (n + PPC - 1) / PPC; }
 
-// Block-wide exclusive scan (PLAN_THREADS threads) of 64-bit values; returns the prefix, *total the sum.
+// Block-wide exclusive scan (PLAN_THREADS threads) of 64-bit values; returns the prefix, *total the sum. One instance per
+// plan kernel (isView), so that each kernel has its own warpSums and the full / depth plan keeps its shared-memory layout.
+template <bool isView>
 __device__ uint64_t blockScan(uint64_t v, uint64_t* total) {
     __shared__ uint64_t warpSums[PLAN_THREADS / 32];
     const uint32_t lane = threadIdx.x & 31u, warp = threadIdx.x >> 5;
@@ -63,20 +73,49 @@ __device__ uint64_t blockScan(uint64_t v, uint64_t* total) {
     return prefix;
 }
 
+// The view export's scratch (all null for the full and depth exports). The breadth-first pass writes the record of every
+// reachable node into rec / recNode here; the records the view keeps are then compacted into the plan's rec / recNode.
+struct ViewScratch {
+    const uint8_t* drawn;         // [node index] 1 when kernel_render draws the node (simlod_export_view_flags)
+    SimlodExportNode* rec;        // [record] breadth-first records of every reachable node
+    uint32_t* recNode;            // [record] their node indices
+    uint8_t* mark;                // [record] 1 when a drawn record lies strictly below
+    uint32_t* index;              // [record] position among the kept records
+};
+
+// One thread per node of nodes[]: drawn[n] = whether kernel_render draws node n for the uniforms `u`, by the renderer's own
+// test (lodcut.cuh). The uniforms come by value, as kernel_render receives them. Writes nothing into nodes[].
+extern "C" __global__ void __launch_bounds__(256)
+simlod_export_view_flags(const SimlodNode* __restrict__ nodes, const SimlodStats* __restrict__ stats, const SimlodUniforms u,
+                         uint32_t maxRecords, uint8_t* __restrict__ drawn) {
+    const uint32_t numNodes = min(stats->numNodes, maxRecords);        // more nodes than records: the plan reports it
+    const float cubeSize = cubeSizeOf(u);
+    for (uint32_t n = blockIdx.x * blockDim.x + threadIdx.x; n < numNodes; n += gridDim.x * blockDim.x) {
+        bool visible, large;
+        drawn[n] = nodeDrawn(u, nodes + n, cubeSize, u.boxMin[0], u.boxMin[1], u.boxMin[2], visible, large) ? 1 : 0;
+    }
+}
+
 // depth < 0: full export. Scratch: rec[maxRecords] (SimlodExportNode), recNode[maxRecords] (node index),
 // recItem[maxRecords] (first chunk item of the record's point list; its voxel list follows).
-extern "C" __global__ void __launch_bounds__(PLAN_THREADS)
-simlod_export_plan(const uint8_t* __restrict__ nodes, const SimlodStats* __restrict__ stats, int32_t depth, uint32_t maxRecords,
-                   SimlodExportNode* __restrict__ rec, uint32_t* __restrict__ recNode, uint64_t* __restrict__ recItem,
-                   ExportCtl* __restrict__ ctl) {
+// isView: the view export (depth < 0, view.drawn set). The breadth-first pass covers every reachable node (so an
+// inconsistent image is reported wherever it is), a record is sampled when its node is drawn, and the records kept are
+// the root and the 8 children of every record with a drawn record strictly below it. A template parameter rather than a
+// test of view.drawn, so that the full and depth exports compile to the plan they had before the view existed.
+template <bool isView>
+__device__ __forceinline__ void plan(const uint8_t* __restrict__ nodes, const SimlodStats* __restrict__ stats, int32_t depth,
+                                     uint32_t maxRecords, SimlodExportNode* __restrict__ rec, uint32_t* __restrict__ recNode,
+                                     uint64_t* __restrict__ recItem, ExportCtl* __restrict__ ctl, const ViewScratch& view) {
     __shared__ uint32_t sh_total, sh_error, sh_maxLevel;
     const uint32_t numNodes = stats->numNodes;
     const uint64_t nodesAddr = (uint64_t)nodes;
+    SimlodExportNode* const bRec = isView ? view.rec : rec;           // breadth-first records
+    uint32_t* const bNode = isView ? view.recNode : recNode;
     if (threadIdx.x == 0) {
         sh_total = 1; sh_error = 0; sh_maxLevel = 0;
         if (numNodes == 0 || numNodes > maxRecords) sh_error = EXPORT_ERR_CHILD;
-        recNode[0] = 0;
-        rec[0].parent = -1;
+        bNode[0] = 0;
+        bRec[0].parent = -1;
     }
     __syncthreads();
     if (sh_error) { if (threadIdx.x == 0) ctl->error = sh_error; return; }
@@ -99,7 +138,7 @@ simlod_export_plan(const uint8_t* __restrict__ nodes, const SimlodStats* __restr
             uint64_t child[8];
             const SimlodNode* node = nullptr;
             if (valid) {
-                node = (const SimlodNode*)(nodes + (uint64_t)recNode[r] * sizeof(SimlodNode));
+                node = (const SimlodNode*)(nodes + (uint64_t)bNode[r] * sizeof(SimlodNode));
                 #pragma unroll
                 for (int k = 0; k < 8; k++) {
                     child[k] = (uint64_t)node->children[k];
@@ -113,7 +152,7 @@ simlod_export_plan(const uint8_t* __restrict__ nodes, const SimlodStats* __restr
             }
             const bool inner = numChildren == 8;
             uint64_t total = 0;
-            const uint32_t pos = (uint32_t)blockScan(valid && expand && inner && !err ? 8 : 0, &total);
+            const uint32_t pos = (uint32_t)blockScan<isView>(valid && expand && inner && !err ? 8 : 0, &total);
             const uint32_t first = sh_total + pos;
             __syncthreads();
             if (threadIdx.x == 0) {
@@ -126,16 +165,16 @@ simlod_export_plan(const uint8_t* __restrict__ nodes, const SimlodStats* __restr
                 if (addChildren) {
                     #pragma unroll
                     for (int k = 0; k < 8; k++) {
-                        recNode[first + k] = (uint32_t)((child[k] - nodesAddr) / sizeof(SimlodNode));
-                        rec[first + k].parent = (int32_t)r;
+                        bNode[first + k] = (uint32_t)((child[k] - nodesAddr) / sizeof(SimlodNode));
+                        bRec[first + k].parent = (int32_t)r;
                     }
                 }
                 // what this record contributes: everything (full), the voxels of an inner node at the cut level, the
-                // points of a leaf at or above it
+                // points of a leaf at or above it; for the view, both lists of a drawn node and nothing else
                 const uint32_t np = node->numPoints, nv = node->numVoxelsStored;
                 const bool full = depth < 0;
-                const bool sampled = full || !inner || level == depth;
-                SimlodExportNode& o = rec[r];
+                const bool sampled = isView ? view.drawn[bNode[r]] != 0 : full || !inner || level == depth;
+                SimlodExportNode& o = bRec[r];
                 o.level = node->level; o.X = node->X; o.Y = node->Y; o.Z = node->Z;
                 const uint32_t* nm = (const uint32_t*)node->name;
                 uint32_t* onm = (uint32_t*)o.name;
@@ -143,8 +182,8 @@ simlod_export_plan(const uint8_t* __restrict__ nodes, const SimlodStats* __restr
                 for (int k = 0; k < 5; k++) onm[k] = nm[k];
                 o.flags = (inner ? 0u : (uint32_t)SIMLOD_EXPORT_LEAF) | (sampled ? (uint32_t)SIMLOD_EXPORT_SAMPLED : 0u);
                 o.first_child = addChildren ? (int32_t)first : -1;
-                o.num_points = full || !inner ? np : 0;
-                o.num_voxels = full || (inner && level == depth) ? nv : 0;
+                o.num_points = (!isView || sampled) && (full || !inner) ? np : 0;
+                o.num_voxels = (!isView || sampled) && (full || (inner && level == depth)) ? nv : 0;
             }
             __syncthreads();
             if (sh_error) break;
@@ -156,18 +195,63 @@ simlod_export_plan(const uint8_t* __restrict__ nodes, const SimlodStats* __restr
     __syncthreads();
     if (sh_error) { if (threadIdx.x == 0) ctl->error = sh_error; return; }
 
+    uint32_t n = sh_total;
+    if (isView) {
+        // |D|: the nodes of nodes[] the renderer draws
+        uint32_t numDrawn = 0;
+        for (uint32_t i = threadIdx.x; i < numNodes; i += PLAN_THREADS) numDrawn += view.drawn[i];
+        uint64_t drawnTotal = 0;
+        blockScan<isView>(numDrawn, &drawnTotal);
+        // mark the ancestors of every drawn record, walking up the parent links (parents precede their children, so a
+        // walk ends at the root within 20 steps). The stores are idempotent; a walk stops at a record another thread has
+        // marked, since that thread goes on to the root.
+        for (uint32_t r = threadIdx.x; r < n; r += PLAN_THREADS) view.mark[r] = 0;
+        __syncthreads();
+        for (uint32_t r = threadIdx.x; r < n; r += PLAN_THREADS)
+            if (view.rec[r].flags & SIMLOD_EXPORT_SAMPLED)
+                for (int32_t p = view.rec[r].parent; p >= 0 && !view.mark[p]; p = view.rec[p].parent) view.mark[p] = 1;
+        __syncthreads();
+        // keep the root and every child of a marked record: whole sibling groups, in breadth-first order. Every drawn
+        // record's parent is marked, so all of them are kept; a drawn node the pass did not reach (or reached twice)
+        // shows as a count other than |D|.
+        uint32_t kept = 0, keptDrawn = 0;
+        for (uint32_t tile = 0; tile < n; tile += PLAN_THREADS) {
+            const uint32_t r = tile + threadIdx.x;
+            bool keep = false;
+            if (r < n) { const int32_t p = view.rec[r].parent; keep = p < 0 || view.mark[p]; }
+            uint64_t total = 0;
+            const uint32_t pos = (uint32_t)blockScan<isView>(keep ? 1 : 0, &total);
+            if (keep) view.index[r] = kept + pos;
+            kept += (uint32_t)total;
+            keptDrawn += (uint32_t)__syncthreads_count(keep && (view.rec[r].flags & SIMLOD_EXPORT_SAMPLED));
+        }
+        if (keptDrawn != drawnTotal) { if (threadIdx.x == 0) ctl->error = EXPORT_ERR_CHILD; return; }
+        // the kept records at their positions, parent and first_child remapped (first_child only on marked records)
+        for (uint32_t r = threadIdx.x; r < n; r += PLAN_THREADS) {
+            const int32_t p = view.rec[r].parent;
+            if (p >= 0 && !view.mark[p]) continue;
+            SimlodExportNode o = view.rec[r];
+            o.parent = p < 0 ? -1 : (int32_t)view.index[p];
+            o.first_child = view.mark[r] ? (int32_t)view.index[o.first_child] : -1;
+            const uint32_t k = view.index[r];
+            rec[k] = o;
+            recNode[k] = view.recNode[r];
+        }
+        n = kept;
+        __syncthreads();
+    }
+
     // sample offsets and chunk items: exclusive scans over the records
-    const uint32_t n = sh_total;
     uint64_t samplesBase = 0, itemsBase = 0, points = 0, voxels = 0;
     for (uint32_t tile = 0; tile < n; tile += PLAN_THREADS) {
         const uint32_t r = tile + threadIdx.x;
         uint32_t np = 0, nv = 0;
         if (r < n) { np = rec[r].num_points; nv = rec[r].num_voxels; }
         uint64_t tS = 0, tI = 0, tP = 0, tV = 0;
-        const uint64_t s = blockScan((uint64_t)np + nv, &tS);
-        const uint64_t it = blockScan(ceilChunks(np) + ceilChunks(nv), &tI);
-        blockScan(np, &tP);
-        blockScan(nv, &tV);
+        const uint64_t s = blockScan<isView>((uint64_t)np + nv, &tS);
+        const uint64_t it = blockScan<isView>(ceilChunks(np) + ceilChunks(nv), &tI);
+        blockScan<isView>(np, &tP);
+        blockScan<isView>(nv, &tV);
         if (r < n) { rec[r].sample_offset = samplesBase + s; recItem[r] = itemsBase + it; }
         samplesBase += tS; itemsBase += tI; points += tP; voxels += tV;
     }
@@ -176,6 +260,21 @@ simlod_export_plan(const uint8_t* __restrict__ nodes, const SimlodStats* __restr
         ctl->numSamples = samplesBase; ctl->numPoints = points; ctl->numVoxels = voxels;
         ctl->numItems = itemsBase; ctl->error = 0;
     }
+}
+
+extern "C" __global__ void __launch_bounds__(PLAN_THREADS)
+simlod_export_plan(const uint8_t* __restrict__ nodes, const SimlodStats* __restrict__ stats, int32_t depth, uint32_t maxRecords,
+                   SimlodExportNode* __restrict__ rec, uint32_t* __restrict__ recNode, uint64_t* __restrict__ recItem,
+                   ExportCtl* __restrict__ ctl) {
+    plan<false>(nodes, stats, depth, maxRecords, rec, recNode, recItem, ctl, ViewScratch{});
+}
+
+// the plan of the view export: depth < 0, the drawn flags of simlod_export_view_flags in view.drawn
+extern "C" __global__ void __launch_bounds__(PLAN_THREADS)
+simlod_export_plan_view(const uint8_t* __restrict__ nodes, const SimlodStats* __restrict__ stats, uint32_t maxRecords,
+                        SimlodExportNode* __restrict__ rec, uint32_t* __restrict__ recNode, uint64_t* __restrict__ recItem,
+                        ExportCtl* __restrict__ ctl, const ViewScratch view) {
+    plan<true>(nodes, stats, -1, maxRecords, rec, recNode, recItem, ctl, view);
 }
 
 // Walks `count` samples' worth of chunks of the list at `head`. Every chunk must lie inside the used heap

@@ -154,7 +154,8 @@ struct SimlodContext {
     CUfunction fnLas = nullptr;
     CUdeviceptr lasStaging = 0;        // raw LAS records of the batch being decoded
     CUmodule exportModule = nullptr;
-    CUfunction fnExportPlan = nullptr, fnExportCollect = nullptr, fnExportGather = nullptr;
+    CUfunction fnExportPlan = nullptr, fnExportCollect = nullptr, fnExportGather = nullptr, fnExportViewFlags = nullptr,
+               fnExportPlanView = nullptr;
     CUdeviceptr exportScratch = 0;     // octree export: records | node indices | first items | chunk items | ExportCtl
     uint64_t exportScratchBytes = 0;
     void* hExportCtl = nullptr;        // pinned copy of ExportCtl
@@ -442,6 +443,8 @@ static int createResources(SimlodContext* ctx, const SimlodConfig* config) {
     CU(D(cuModuleGetFunction)(&ctx->fnExportPlan, ctx->exportModule, "simlod_export_plan"));
     CU(D(cuModuleGetFunction)(&ctx->fnExportCollect, ctx->exportModule, "simlod_export_collect"));
     CU(D(cuModuleGetFunction)(&ctx->fnExportGather, ctx->exportModule, "simlod_export_gather"));
+    CU(D(cuModuleGetFunction)(&ctx->fnExportViewFlags, ctx->exportModule, "simlod_export_view_flags"));
+    CU(D(cuModuleGetFunction)(&ctx->fnExportPlanView, ctx->exportModule, "simlod_export_plan_view"));
 
     // buffers (main.cpp:552-586)
     SimlodBuffers& b = ctx->buf;
@@ -1124,7 +1127,7 @@ int simlod_flush_l2(SimlodContext* ctx) {
     return SIMLOD_OK;
 }
 
-// ---- octree export (DESIGN.md §9.4); kernels in export.cu -------------------------------------------------
+// ---- octree export (DESIGN.md §9.4, §9.5); kernels in export.cu --------------------------------------------
 namespace {
 struct ExportCtl {                   // mirrors export.cu
     uint32_t numNodes, maxLevel;
@@ -1132,20 +1135,28 @@ struct ExportCtl {                   // mirrors export.cu
     uint64_t numItems;
     uint32_t error, pad;
 };
+struct ExportViewScratch {           // mirrors export.cu ViewScratch
+    CUdeviceptr drawn, rec, recNode, mark, index;
+};
 constexpr uint64_t align16(uint64_t v) { return (v + 15) & ~15ull; }
-}  // namespace
 
-int simlod_export_octree(SimlodContext* ctx, int32_t depth, uint64_t dst_nodes, uint64_t node_capacity,
-                         uint64_t dst_samples, uint64_t sample_capacity, SimlodExportInfo* info, float* kernel_ms) {
+// The export of simlod_export_octree (view == nullptr) and simlod_export_view (the LOD cut for *view).
+int exportOctree(SimlodContext* ctx, int32_t depth, const SimlodUniforms* view, uint64_t dst_nodes, uint64_t node_capacity,
+                 uint64_t dst_samples, uint64_t sample_capacity, SimlodExportInfo* info, float* kernel_ms) {
     int rc = setCurrent(ctx); if (rc) return rc;
     if (!info) return fail(SIMLOD_ERR_INVALID, "null info");
     if (depth > SIMLOD_MAX_DEPTH) return fail(SIMLOD_ERR_INVALID, "export depth %d exceeds the octree's maximum depth %d", depth, (int)SIMLOD_MAX_DEPTH);
     if (dst_nodes % 16 || dst_samples % 16) return fail(SIMLOD_ERR_INVALID, "export destinations must be 16-byte aligned");
-    // scratch, sized by the context's buffers: one record per node of nodes[], one item per chunk the heap can hold
+    // scratch, sized by the context's buffers: one record per node of nodes[], one item per chunk the heap can hold; the
+    // view adds per node a drawn byte, and per record a mark byte, an index and a second record and node index
     const uint32_t maxRecords = (uint32_t)(ctx->buf.nodes_bytes / sizeof(SimlodNode));
     const uint64_t itemsCap = ctx->buf.persistent_bytes / SIMLOD_CHUNK_STRIDE + 1;
     const uint64_t offNode = align16((uint64_t)maxRecords * sizeof(SimlodExportNode)), offItem = offNode + align16((uint64_t)maxRecords * 4),
-                   offItems = offItem + align16((uint64_t)maxRecords * 8), offCtl = offItems + itemsCap * 16, bytes = offCtl + sizeof(ExportCtl);
+                   offItems = offItem + align16((uint64_t)maxRecords * 8), offCtl = offItems + itemsCap * 16,
+                   offDrawn = align16(offCtl + sizeof(ExportCtl)), offMark = offDrawn + align16(maxRecords),
+                   offIndex = offMark + align16(maxRecords), offViewRec = offIndex + align16((uint64_t)maxRecords * 4),
+                   offViewNode = offViewRec + align16((uint64_t)maxRecords * sizeof(SimlodExportNode)),
+                   bytes = view ? offViewNode + align16((uint64_t)maxRecords * 4) : offCtl + sizeof(ExportCtl);
     if (ctx->exportScratchBytes < bytes) {
         if (ctx->exportScratch) CU(D(cuMemFree)(ctx->exportScratch));
         ctx->exportScratch = 0;
@@ -1156,11 +1167,25 @@ int simlod_export_octree(SimlodContext* ctx, int32_t depth, uint64_t dst_nodes, 
     if (!ctx->hExportCtl) CU(D(cuMemHostAlloc)(&ctx->hExportCtl, sizeof(ExportCtl), 0));
     CUdeviceptr nodes = ctx->buf.nodes, heap = ctx->buf.persistent, stats = ctx->buf.stats;
     CUdeviceptr rec = ctx->exportScratch, recNode = rec + offNode, recItem = rec + offItem, items = rec + offItems, ctl = rec + offCtl;
+    ExportViewScratch vs{};
+    if (view) vs = ExportViewScratch{rec + offDrawn, rec + offViewRec, rec + offViewNode, rec + offMark, rec + offIndex};
     uint64_t heapBytes = ctx->buf.persistent_bytes;
-    // stage 1: plan (one block) and the chunk-list walk, both into scratch only
+    // stage 1: the view's drawn flags (one thread per node), plan (one block) and the chunk-list walk, all into scratch only
     CU(D(cuEventRecord)(ctx->evStart, ctx->streamMain));
-    { void* args[] = {&nodes, &stats, &depth, (void*)&maxRecords, &rec, &recNode, &recItem, &ctl};
-      CU(D(cuLaunchKernel)(ctx->fnExportPlan, 1, 1, 1, 1024, 1, 1, 0, ctx->streamMain, args, nullptr)); }
+    if (view) {
+        SimlodUniforms u = *view;
+        CUdeviceptr drawn = vs.drawn;
+        void* args[] = {&nodes, &stats, &u, (void*)&maxRecords, &drawn};
+        CU(D(cuLaunchKernel)(ctx->fnExportViewFlags, (unsigned)ctx->numSMs * 4, 1, 1, 256, 1, 1, 0, ctx->streamMain, args, nullptr));
+        ctx->launches++;
+    }
+    if (view) {
+        void* args[] = {&nodes, &stats, (void*)&maxRecords, &rec, &recNode, &recItem, &ctl, &vs};
+        CU(D(cuLaunchKernel)(ctx->fnExportPlanView, 1, 1, 1, 1024, 1, 1, 0, ctx->streamMain, args, nullptr));
+    } else {
+        void* args[] = {&nodes, &stats, &depth, (void*)&maxRecords, &rec, &recNode, &recItem, &ctl};
+        CU(D(cuLaunchKernel)(ctx->fnExportPlan, 1, 1, 1, 1024, 1, 1, 0, ctx->streamMain, args, nullptr));
+    }
     uint64_t cap = itemsCap;
     { void* args[] = {&nodes, &heap, &heapBytes, &rec, &recNode, &recItem, &items, &cap, &ctl};
       CU(D(cuLaunchKernel)(ctx->fnExportCollect, (unsigned)ctx->numSMs * 2, 1, 1, 256, 1, 1, 0, ctx->streamMain, args, nullptr)); }
@@ -1193,6 +1218,18 @@ int simlod_export_octree(SimlodContext* ctx, int32_t depth, uint64_t dst_nodes, 
     CU(D(cuEventElapsedTime)(&gatherMs, ctx->evTotalStart, ctx->evTotalEnd));
     if (kernel_ms) *kernel_ms = ms + gatherMs;
     return SIMLOD_OK;
+}
+}  // namespace
+
+int simlod_export_octree(SimlodContext* ctx, int32_t depth, uint64_t dst_nodes, uint64_t node_capacity,
+                         uint64_t dst_samples, uint64_t sample_capacity, SimlodExportInfo* info, float* kernel_ms) {
+    return exportOctree(ctx, depth, nullptr, dst_nodes, node_capacity, dst_samples, sample_capacity, info, kernel_ms);
+}
+
+int simlod_export_view(SimlodContext* ctx, uint64_t dst_nodes, uint64_t node_capacity, uint64_t dst_samples,
+                       uint64_t sample_capacity, SimlodExportInfo* info, float* kernel_ms) {
+    if (!ctx) return fail(SIMLOD_ERR_INVALID, "null context");
+    return exportOctree(ctx, -1, &ctx->uniforms, dst_nodes, node_capacity, dst_samples, sample_capacity, info, kernel_ms);
 }
 
 // ---- spatial exchange (SURVEY.md §8f-3); kernels in partition.cu ----------------------------------------
