@@ -89,7 +89,12 @@ typedef struct SimlodUniforms {
     uint64_t   frameCounter;               // 416
     float      boxMin[3];                  // 424
     float      boxMax[3];                  // 436
-    uint8_t    showBoundingBox;            // 448
+    uint8_t    showBoundingBox;            // 448 nonzero: kernel_render draws, after the samples and before EDL, the
+                                           //     frustum of transformInv_updateBound (8 lines, colour 0x000000ff) and
+                                           //     the box of every drawn node (12 lines, 0x0000ff00), 1-pixel lines
+                                           //     clipped to and projected by `transform`, depth-tested by atomicMin
+                                           //     (the reference's frame; above 10 416 drawn nodes, where the reference
+                                           //     overruns its line list, every box is still drawn)
     uint8_t    showPoints;                 // 449
     uint8_t    colorByNode;                // 450
     uint8_t    colorByLOD;                 // 451

@@ -42,6 +42,18 @@ __device__ __forceinline__ float lg2(float a) {          // MUFU.LG2
 __device__ __forceinline__ float sqrt_approx(float a) {  // MUFU.SQRT
     float r; asm("sqrt.approx.ftz.f32 %0, %1;" : "=f"(r) : "f"(a)); return r;
 }
+__device__ __forceinline__ float rsqrt(float a) {        // MUFU.RSQ
+    float r; asm("rsqrt.approx.ftz.f32 %0, %1;" : "=f"(r) : "f"(a)); return r;
+}
+__device__ __forceinline__ float rcp_rn(float a) {       // MUFU.RCP + Newton step, correctly rounded (float(1.0 / double(a)))
+    float r; asm("rcp.rn.f32 %0, %1;" : "=f"(r) : "f"(a)); return r;
+}
+__device__ __forceinline__ float min_ftz(float a, float b) {   // FMNMX.FTZ: a NaN operand yields the other one
+    float r; asm("min.ftz.f32 %0, %1, %2;" : "=f"(r) : "f"(a), "f"(b)); return r;
+}
+__device__ __forceinline__ float max_ftz(float a, float b) {
+    float r; asm("max.ftz.f32 %0, %1, %2;" : "=f"(r) : "f"(a), "f"(b)); return r;
+}
 // a / b as the reference computes it: a * MUFU.RCP(b), product flushed
 __device__ __forceinline__ float div_fast(float a, float b) { return mul_ftz(a, rcp(b)); }
 
@@ -65,6 +77,12 @@ __device__ __forceinline__ double dadd(double a, double b) {
 }
 __device__ __forceinline__ int32_t d2i(double a) {       // F2I.F64.TRUNC
     int32_t r; asm("cvt.rzi.s32.f64 %0, %1;" : "=r"(r) : "d"(a)); return r;
+}
+__device__ __forceinline__ double f2d(float a) {         // F2F.F64.F32
+    double r; asm("cvt.f64.f32 %0, %1;" : "=d"(r) : "f"(a)); return r;
+}
+__device__ __forceinline__ float d2f(double a) {         // F2F.F32.F64
+    float r; asm("cvt.rn.f32.f64 %0, %1;" : "=f"(r) : "d"(a)); return r;
 }
 
 }  // namespace fpx
