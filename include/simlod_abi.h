@@ -169,6 +169,16 @@ typedef struct SimlodExportInfo {
     uint64_t num_samples, num_points, num_voxels;
 } SimlodExportInfo;
 
+// The LAS public header fields the reference reads (LasLoader.h:21-55), at their file byte offsets:
+typedef struct SimlodLasHeader {
+    uint32_t version_major, version_minor;        // bytes 24, 25 (u8)
+    uint32_t format, bytes_per_point;             // 104 (u8), 105 (u16)
+    uint32_t header_size, offset_to_point_data;   // 94 (u16), 96 (u32)
+    uint64_t num_points;                          // 107 (u32) for versions 1.0-1.3, else 247 (u64)
+    double   scale[3], offset[3];                 // 131, 155
+    double   min[3], max[3];                      // min 187 / 203 / 219, max 179 / 195 / 211
+} SimlodLasHeader;
+
 SIMLOD_STATIC_ASSERT(sizeof(SimlodPoint) == 16, "Point");
 SIMLOD_STATIC_ASSERT(sizeof(SimlodChunk) == 16016, "Chunk");
 SIMLOD_STATIC_ASSERT(offsetof(SimlodChunk, size) == 16000, "Chunk.size");
@@ -218,4 +228,9 @@ SIMLOD_STATIC_ASSERT(offsetof(SimlodExportNode, sample_offset) == 48, "ExportNod
 SIMLOD_STATIC_ASSERT(offsetof(SimlodExportNode, num_points) == 56, "ExportNode.num_points");
 SIMLOD_STATIC_ASSERT(offsetof(SimlodExportNode, num_voxels) == 60, "ExportNode.num_voxels");
 SIMLOD_STATIC_ASSERT(sizeof(SimlodExportInfo) == 32, "ExportInfo");
+SIMLOD_STATIC_ASSERT(sizeof(SimlodLasHeader) == 128, "LasHeader");
+SIMLOD_STATIC_ASSERT(offsetof(SimlodLasHeader, num_points) == 24, "LasHeader.num_points");
+SIMLOD_STATIC_ASSERT(offsetof(SimlodLasHeader, scale) == 32, "LasHeader.scale");
+SIMLOD_STATIC_ASSERT(offsetof(SimlodLasHeader, min) == 80, "LasHeader.min");
+SIMLOD_STATIC_ASSERT(offsetof(SimlodLasHeader, max) == 104, "LasHeader.max");
 SIMLOD_STATIC_ASSERT(offsetof(SimlodExportInfo, num_samples) == 8, "ExportInfo.num_samples");

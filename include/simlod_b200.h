@@ -131,8 +131,32 @@ typedef struct SimlodLasLayout {
     double   offset[3];
     double   translation[3];        // the host passes -min (main.cpp:868-873), so that boxMin = 0
 } SimlodLasLayout;
+// Records from host memory are copied into a ring of device staging slots on a copy stream of their own; the decode
+// waits for its copy, so the copies of later batches keep the PCIe link busy while an update launch occupies the SMs.
 int simlod_upload_batch_las(SimlodContext* ctx, const void* host_records, uint32_t count, const SimlodLasLayout* layout);
 int simlod_upload_batch_las_device(SimlodContext* ctx, uint64_t device_records, uint32_t count, const SimlodLasLayout* layout);
+
+// The LAS public header fields the reference reads (loadHeader, LasLoader.h:21-55); layout in simlod_abi.h.
+// SIMLOD_ERR_INVALID naming the file when it cannot be read, is shorter than its header or lacks the LASF signature.
+// Needs no context and no GPU.
+int simlod_read_las_header(const char* path, SimlodLasHeader* out);
+
+// reload() of the reference for a list of point-cloud files (main.cpp:644-773, 811-958; onFileDrop, :1120-1150):
+// `.las` and `.simlod` files, by extension, compared case-insensitively. Every path, header and file size is checked
+// first; on any error the call returns SIMLOD_ERR_INVALID naming the file and leaves the octree, Stats and uniforms as
+// they were (a missing file, an unknown extension, `.laz`, no LASF signature, a record size or format the decoder
+// rejects, records past the end of the file, a `.simlod` file shorter than its 24-byte header). Then:
+//   box        the union of float(header min / max) of the LAS files and the header floats of the .simlod files;
+//              the uniforms get boxMin = 0, boxMax = max - min (float), and the octree is reset
+//   batches    each file in list order is cut into ceil(n / 1 000 000) batches, the last one partial; a file without
+//              points adds its box and no batch
+//   decode     LAS records are decoded on the device with translation = -boxMin (simlod_upload_batch_las: alpha 0xff,
+//              RGB for formats 2, 3, 5 and 7 only); .simlod points are inserted as they are stored
+// `loader_threads` host threads read ~1 MB pieces of the files in list order into a 512 MB page-locked pool; batches are
+// published in list order. *num_points, *kernel_ms, *total_ms and SIMLOD_STREAM_DIRECT (for every file) as for
+// simlod_insert_simlod_file_ex.
+int simlod_insert_files(SimlodContext* ctx, const char* const* paths, uint32_t num_paths, int loader_threads,
+                        uint32_t flags, uint64_t* num_points, float* kernel_ms, float* total_ms);
 
 // renderCUDA (main.cpp:465-546): one cooperative launch of kernel_render into the surface.
 int simlod_render(SimlodContext* ctx, float* kernel_ms);

@@ -99,6 +99,16 @@ class LasLayout(C.Structure):
                 ("translation", C.c_double * 3)]
 
 
+class LasHeader(C.Structure):
+    """SimlodLasHeader: the LAS public header fields the reference reads (LasLoader.h:21-55), 128 bytes."""
+    _fields_ = [("version_major", C.c_uint32), ("version_minor", C.c_uint32), ("format", C.c_uint32), ("bytes_per_point", C.c_uint32),
+                ("header_size", C.c_uint32), ("offset_to_point_data", C.c_uint32), ("num_points", C.c_uint64),
+                ("scale", C.c_double * 3), ("offset", C.c_double * 3), ("min", C.c_double * 3), ("max", C.c_double * 3)]
+
+    def as_dict(self):
+        return {f: (tuple(getattr(self, f)) if f in ("scale", "offset", "min", "max") else int(getattr(self, f))) for f, _ in self._fields_}
+
+
 class PartitionPlan(C.Structure):
     """SimlodPartitionPlan: the level-`level` cells of the octree cube and the rank that owns each."""
     _fields_ = [("level", C.c_uint32), ("num_ranks", C.c_uint32), ("owner", C.c_uint8 * 512)]
@@ -126,6 +136,7 @@ class OctreeExport:
 
 assert C.sizeof(Uniforms) == 480 and C.sizeof(Stats) == 112
 assert C.sizeof(ExportInfo) == 32 and EXPORT_NODE_DTYPE.itemsize == 64
+assert C.sizeof(LasHeader) == 128
 
 # every symbol include/simlod_b200.h declares
 EXPORTS = [
@@ -137,7 +148,7 @@ EXPORTS = [
     "simlod_get_launch_info", "simlod_device_rcp", "simlod_synchronize", "simlod_flush_l2",
     "simlod_partition_count", "simlod_partition_scatter", "simlod_partition_wait",
     "simlod_export_framebuffer", "simlod_peer_signal", "simlod_composite_framebuffers", "simlod_generate", "simlod_reset_with_grid", "simlod_insert_simlod_file_ex", "simlod_get_numa_node",
-    "simlod_export_octree", "simlod_export_view",
+    "simlod_export_octree", "simlod_export_view", "simlod_read_las_header", "simlod_insert_files",
 ]
 
 _lib = None
@@ -195,6 +206,8 @@ def load_library():
         "simlod_composite_framebuffers": [vp, C.POINTER(u64), u32, u32, C.POINTER(u64), u32],
         "simlod_export_octree": [vp, C.c_int32, u64, u64, u64, u64, C.POINTER(ExportInfo), C.POINTER(C.c_float)],
         "simlod_export_view": [vp, u64, u64, u64, u64, C.POINTER(ExportInfo), C.POINTER(C.c_float)],
+        "simlod_read_las_header": [C.c_char_p, C.POINTER(LasHeader)],
+        "simlod_insert_files": [vp, C.POINTER(C.c_char_p), u32, C.c_int, u32, C.POINTER(u64), C.POINTER(C.c_float), C.POINTER(C.c_float)],
     }
     for name, argtypes in sig.items():
         fn = getattr(lib, name)
@@ -202,6 +215,17 @@ def load_library():
         fn.restype = None if name == "simlod_destroy" else C.c_int
     _lib = lib
     return lib
+
+
+def read_las_header(path):
+    """The header fields of a LAS file as the reference's loadHeader reads them (simlod_read_las_header): a LasHeader
+    (`.as_dict()` for a plain dict). Needs no GPU. Raises SimlodError(-2) naming the file when it is not a LAS file."""
+    lib = load_library()
+    h = LasHeader()
+    rc = lib.simlod_read_las_header(os.fsencode(path), C.byref(h))
+    if rc != 0:
+        raise SimlodError(rc, lib.simlod_last_error().decode())
+    return h
 
 
 def make_points(xyz, color):
@@ -376,6 +400,19 @@ class SimLOD:
         n, kms, tms = C.c_uint64(), C.c_float(), C.c_float()
         self._check(self._lib.simlod_insert_simlod_file_ex(self._ctx, path.encode(), int(loader_threads), 1 if direct else 0, C.byref(n), C.byref(kms), C.byref(tms)))
         self._lib.simlod_get_uniforms(self._ctx, C.byref(self.uniforms))
+        return n.value, kms.value, tms.value
+
+    def insert_files(self, paths, loader_threads=16, direct=False):
+        """reload() of the reference for a list of .las / .simlod files (simlod_insert_files): validate every file (on
+        error nothing changes), set the union box, reset, and stream the files' 1 M-point batches in list order, LAS
+        records decoded on the device. direct=True reads unbuffered (O_DIRECT). Returns (num_points, summed kernel ms,
+        total device ms)."""
+        paths = [os.fsencode(p) for p in paths]
+        arr = (C.c_char_p * max(1, len(paths)))(*paths)
+        n, kms, tms = C.c_uint64(), C.c_float(), C.c_float()
+        rc = self._lib.simlod_insert_files(self._ctx, arr, len(paths), int(loader_threads), 1 if direct else 0, C.byref(n), C.byref(kms), C.byref(tms))
+        self._lib.simlod_get_uniforms(self._ctx, C.byref(self.uniforms))
+        self._check(rc)
         return n.value, kms.value, tms.value
 
     def insert_batches(self, batches):
