@@ -213,7 +213,7 @@ struct Ctx {
     __device__ __forceinline__ Point*     spilled()     const { return at<Point>(scratch::OFF_SPILLED); }
     __device__ __forceinline__ uint64_t*  vkey(uint32_t p)   const { return at<uint64_t>(scratch::OFF_VKEY) + p * scratch::VOXEL_CAP; }     // cell | node << 21 | slot << 41
     __device__ __forceinline__ uint32_t*  vcolor(uint32_t p) const { return at<uint32_t>(scratch::OFF_VCOLOR) + p * scratch::VOXEL_CAP; }
-    __device__ __forceinline__ uint32_t*  worklist()    const { return at<uint32_t>(scratch::OFF_WORKLIST); }    // items (leafOf index) the coming re-walk pass visits
+    __device__ __forceinline__ uint32_t*  worklist()    const { return at<uint32_t>(scratch::OFF_WORKLIST); }    // items the coming re-walk pass visits (leafOf index | split << 22)
 };
 
 // the batch a pass works on
@@ -493,7 +493,12 @@ constexpr uint32_t LIST_CAP = 2048;
 __shared__ uint32_t sh_listCount;         // entries of the explicit list (may run past LIST_CAP: overflow)
 __shared__ uint32_t sh_listMode;          // 0: the run (sh_runSlot), 1: the explicit list
 __shared__ uint32_t sh_blockLegacy;       // this block cannot name its items any more in this batch
-__shared__ uint8_t  sh_entrySplit[VOXTAB_SIZE];
+__shared__ uint8_t  sh_entrySplit[VOXTAB_SIZE];   // split phase: table entry -> 1 + index of its leaf among the round's splits (0: not split)
+// A worklist entry names the item (leafOf / slotOf index) and the split it moves out of: item | split << 22. Worklist
+// rounds split at most 64 leaves, so the split takes 6 bits and no entry reaches 0xffffffff.
+constexpr uint32_t WL_SPLIT_SHIFT = 22;
+constexpr uint32_t WL_ITEM_MASK = (1u << WL_SPLIT_SHIFT) - 1u;
+static_assert(scratch::ITEM_CAP <= (1u << WL_SPLIT_SHIFT), "worklist entries keep the item in 22 bits");
 __shared__ uint32_t sh_splitNodes[64];
 __shared__ SpillInfo sh_splitInfo[64];       // the leaves split in the current round (worklist rounds: at most 64) ...
 __shared__ uint32_t sh_splitGranule[65];     // ... and the running number of 32-point granules of their spilled points
@@ -853,12 +858,13 @@ __device__ void buildWorklist(const Ctx& c, const Batch& b, uint32_t spillBegin,
     if (threadIdx.x < VOXTAB_SIZE) {
         const uint32_t key = sh_leafKey[threadIdx.x];
         uint32_t f = 0;
-        if (key != VOXTAB_EMPTY) for (uint32_t j = 0; j < numSplit; j++) f |= key == sh_splitNodes[j] ? 1u : 0u;
+        if (key != VOXTAB_EMPTY) for (uint32_t j = 0; j < numSplit; j++) f = key == sh_splitNodes[j] ? j + 1u : f;
         sh_entrySplit[threadIdx.x] = (uint8_t)f;
     }
     __syncthreads();
     const uint32_t* words = mode == 0 ? sh_runSlot : listSlot();
     auto movedAt = [&](uint32_t k) { const uint32_t word = words[k]; return (word & PROVISIONAL) != 0 && sh_entrySplit[(word >> 24) & (VOXTAB_SIZE - 1)] != 0; };
+    auto wlSplit = [&](uint32_t word) { return (uint32_t)(sh_entrySplit[(word >> 24) & (VOXTAB_SIZE - 1)] - 1u) << WL_SPLIT_SHIFT; };
     uint32_t cnt = 0;
     for (uint32_t k = threadIdx.x; k < total; k += blockDim.x) cnt += movedAt(k) ? 1u : 0u;
     for (int o = 16; o > 0; o >>= 1) cnt += __shfl_xor_sync(0xffffffffu, cnt, o);
@@ -883,7 +889,7 @@ __device__ void buildWorklist(const Ctx& c, const Batch& b, uint32_t spillBegin,
         uint32_t off = 0;
         if (laneId() == 0) off = atomicAdd(&sh_wlFill, (uint32_t)__popc(mask));
         off = __shfl_sync(0xffffffffu, off, 0);
-        if (m) wl[base + off + __popc(mask & lanemaskLt())] = mode == 0 ? blockFirst + k : items[k];
+        if (m) wl[base + off + __popc(mask & lanemaskLt())] = (mode == 0 ? blockFirst + k : items[k]) | wlSplit(words[k]);
     }
 }
 
@@ -940,9 +946,8 @@ __device__ __forceinline__ void passItems(const Ctx& c, const Batch& b, uint32_t
         uint32_t* slotOf = c.slotOf(b.parity);
         if (sh_roundLegacy == 0) {
             // ---- the items the split phase named (buildWorklist), then the points spilled in this round ---------------------
-            const uint32_t numListed = min(sh_roundListed, (uint32_t)scratch::WL_CAP);
+            const uint32_t listed = min(sh_roundListed, (uint32_t)scratch::WL_CAP);
             const uint32_t perRun = ((b.size + gridDim.x - 1) / gridDim.x + 31u) & ~31u;
-            const uint32_t* wl = c.worklist();
             const uint32_t numSplit = spillEnd - spillBegin;                      // <= 64 in worklist rounds
             if (threadIdx.x < numSplit) sh_splitInfo[threadIdx.x] = c.spill()[spillBegin + threadIdx.x];
             if (threadIdx.x == 0) { sh_listCount = 0; sh_listMode = 1; }          // the list of the previous round has been read (split phase)
@@ -980,11 +985,13 @@ __device__ __forceinline__ void passItems(const Ctx& c, const Batch& b, uint32_t
             RW_DONE(12);
             // ---- (1) the items the split phase named (buildWorklist): batch points, and points spilled in earlier rounds. Each sits
             // in a leaf that was split in THIS round (that is how it got on the list), so the step down is the same as in (2):
-            // the leaf's record gives the children and the only grid to sample
-            // Both loops are software-pipelined: a granule's work is a chain of dependent loads (list entry -> leaf word and
-            // point -> grid word -> atomic), and a warp has only a handful of granules, so the list entry two granules ahead and
-            // the leaf word + point one granule ahead are in flight while a granule is processed. The grid of the split leaf comes
-            // from its record (no side-table load).
+            // the leaf's record, which the entry names, gives the node, level, children and the only grid to sample.
+            // Both loops hand each block a contiguous share of their items: the worklist is the blocks' segments of the
+            // batch one after another, so a share holds the items of a few runs and a few split leaves, and the block's
+            // table sees few children (one global add each at the flush, and room left to name the next round's items).
+            // Both loops are software-pipelined: a granule's work is a chain of dependent loads (list entry -> point -> grid
+            // word -> atomic), and a warp has only a handful of granules, so the list entry two granules ahead and the point
+            // one granule ahead are in flight while a granule is processed.
             constexpr uint32_t NO_ITEM = 0xffffffffu;
             auto sampleSplitLeaf = [&](uint64_t grid, const Coords& q, uint32_t color, uint32_t node, uint32_t level) {
                 if (!nested(q)) atomicOr(&c.ctl()->errorFlags, ERR_FAR_POINT);         // (as sampleUp flags it)
@@ -995,35 +1002,33 @@ __device__ __forceinline__ void passItems(const Ctx& c, const Batch& b, uint32_t
                 if ((seen & bit) == 0 && (atomicOr(word, bit) & bit) == 0) recordVoxel(c, b, node, cell, color);
             };
             {
-                const uint32_t stride = rewalkGranuleStride();
-                auto loadIndex = [&](uint32_t bs) { const uint32_t u = bs + laneId(); return (bs < numListed && u < numListed) ? wl[u] : NO_ITEM; };
-                auto loadItem = [&](uint32_t i, uint32_t& lp, uint4& pt) {
-                    lp = 0; pt = make_uint4(0, 0, 0, 0);
-                    if (i != NO_ITEM) {
-                        pt = i >= scratch::MAX_BATCH ? *reinterpret_cast<const uint4*>(c.spilled() + (i - scratch::MAX_BATCH)) : ldPoint(b.points + i);
-                        lp = leafOf[i];
-                    }
+                // block k visits the entries [k * share, (k + 1) * share) of the list, its warps consecutive granules of it
+                const uint32_t share = ((listed + gridDim.x - 1) / gridDim.x + 31u) & ~31u;
+                const uint32_t first = min(listed, blockIdx.x * share);
+                const uint32_t numListed = min(listed - first, share);               // the entries of this block's share
+                const uint32_t* wl = c.worklist() + first;
+                const uint32_t stride = blockDim.x;
+                auto loadEntry = [&](uint32_t bs) { const uint32_t u = bs + laneId(); return u < numListed ? wl[u] : NO_ITEM; };
+                auto loadPoint = [&](uint32_t e) {
+                    const uint32_t i = e & WL_ITEM_MASK;
+                    if (e == NO_ITEM) return make_uint4(0, 0, 0, 0);
+                    return i >= scratch::MAX_BATCH ? *reinterpret_cast<const uint4*>(c.spilled() + (i - scratch::MAX_BATCH)) : ldPoint(b.points + i);
                 };
-                uint32_t base = rewalkFirstGranule();
-                uint32_t iCur = loadIndex(base), iNext = loadIndex(base + stride);
-                uint32_t lpCur; uint4 ptCur;
-                loadItem(iCur, lpCur, ptCur);
+                uint32_t base = threadIdx.x & ~31u;
+                uint32_t eCur = loadEntry(base), eNext = loadEntry(base + stride);
+                uint4 ptCur = loadPoint(eCur);
                 for (; base < numListed; base += stride) {
-                    uint32_t lpNext; uint4 ptNext;
-                    loadItem(iNext, lpNext, ptNext);                                   // granule base + stride
-                    const uint32_t iNext2 = loadIndex(base + 2u * stride);
-                    const uint32_t i = iCur;
+                    const uint4 ptNext = loadPoint(eNext);                               // granule base + stride
+                    const uint32_t eNext2 = loadEntry(base + 2u * stride);
+                    const uint32_t i = eCur & WL_ITEM_MASK, k = eCur >> WL_SPLIT_SHIFT;
                     const uint4 pt = ptCur;
-                    bool valid = i != NO_ITEM;
+                    bool valid = eCur != NO_ITEM;
                     const bool spilledItem = valid && i >= scratch::MAX_BATCH;
                     uint32_t node = 0, level = 0, childBase = 0;
                     uint64_t grid = 0;
                     if (valid) {
-                        node = lpCur & 0xffffffu; level = lpCur >> 24;
-                        uint32_t k = 0;
-                        while (k < numSplit && sh_splitInfo[k].node != node) k++;
-                        if (k < numSplit) { childBase = sh_splitInfo[k].childBase; grid = sh_splitInfo[k].grid; }
-                        else { valid = false; atomicOr(&c.ctl()->errorFlags, ERR_INTERNAL); }      // cannot happen: listed items sit in split leaves
+                        if (k < numSplit) { node = sh_splitInfo[k].node; level = sh_splitInfo[k].level; childBase = sh_splitInfo[k].childBase; grid = sh_splitInfo[k].grid; }
+                        else { valid = false; atomicOr(&c.ctl()->errorFlags, ERR_INTERNAL); }      // cannot happen: the split phase names one of this round's splits
                         valid = valid && level < SIMLOD_MAX_DEPTH;               // a level-20 node is the leaf even after it "split" (voxels.cu:169)
                     }
                     if (__any_sync(0xffffffffu, valid)) {
@@ -1037,7 +1042,7 @@ __device__ __forceinline__ void passItems(const Ctx& c, const Batch& b, uint32_t
                         if (COUNT) slot = countInto<true>(c, b, valid, child, level + 1, valid && !spilledItem ? c.runBloom() + (i / perRun) * BLOOM_WORDS : nullptr, forceGlobal);
                         if (valid && COUNT) remember(i, child | ((level + 1) << 24), slot, myk, forceGlobal);
                     }
-                    iCur = iNext; lpCur = lpNext; ptCur = ptNext; iNext = iNext2;
+                    eCur = eNext; ptCur = ptNext; eNext = eNext2;
                 }
             }
             RW_DONE(13);
@@ -1045,22 +1050,27 @@ __device__ __forceinline__ void passItems(const Ctx& c, const Batch& b, uint32_t
             // record (children, grid, level) is in shared memory — no leaf look-up, no descent: the child is one step down,
             // the only grid on the way is the leaf's own fresh one
             {
-                const uint32_t numGranules = sh_splitGranule[numSplit];
-                const uint32_t gStride = rewalkGranuleStride() / 32u;
+                // block k takes the granules [k * share, (k + 1) * share), its warps consecutive ones
+                const uint32_t allGranules = sh_splitGranule[numSplit];
+                const uint32_t share = (allGranules + gridDim.x - 1) / gridDim.x;
+                const uint32_t gFirst = min(allGranules, blockIdx.x * share);
+                const uint32_t numGranules = min(allGranules - gFirst, share);      // the granules of this block's share
+                const uint32_t gStride = blockDim.x / 32u;
                 struct Granule { uint32_t lo, j; bool valid; };
                 auto locate = [&](uint32_t g) {
                     Granule r; r.lo = 0; r.j = 0; r.valid = false;
                     if (g < numGranules) {
-                        uint32_t lo = 0, hi = numSplit;                      // last split with first granule <= g
-                        while (hi - lo > 1) { const uint32_t mid = (lo + hi) >> 1; if (sh_splitGranule[mid] <= g) lo = mid; else hi = mid; }
-                        const uint32_t within = (g - sh_splitGranule[lo]) * 32u + laneId();
+                        const uint32_t ga = gFirst + g;
+                        uint32_t lo = 0, hi = numSplit;                      // last split with first granule <= ga
+                        while (hi - lo > 1) { const uint32_t mid = (lo + hi) >> 1; if (sh_splitGranule[mid] <= ga) lo = mid; else hi = mid; }
+                        const uint32_t within = (ga - sh_splitGranule[lo]) * 32u + laneId();
                         r.lo = lo; r.j = sh_splitInfo[lo].base + within;
                         r.valid = within < sh_splitInfo[lo].stored && sh_splitInfo[lo].level < SIMLOD_MAX_DEPTH;
                     }
                     return r;
                 };
                 auto loadSpilled = [&](const Granule& gr) { return gr.valid ? *reinterpret_cast<const uint4*>(c.spilled() + gr.j) : make_uint4(0, 0, 0, 0); };
-                uint32_t g = rewalkFirstGranule() / 32u;
+                uint32_t g = threadIdx.x >> 5;
                 Granule cur = locate(g);
                 uint4 ptCur = loadSpilled(cur);
                 for (; g < numGranules; g += gStride) {

@@ -130,13 +130,15 @@ for K in sizes:
             assert st.numPoints == n and st.dbg == 0, (st.numPoints, st.dbg)
             ph = sim.memcpy_dtoh(sim.buffers().momentary + 96, 64).view(np.uint64).astype(np.float64)
             sub = sim.memcpy_dtoh(sim.buffers().momentary + 800, 128).view(np.uint64).astype(np.float64)
+            ev = sim.memcpy_dtoh(sim.buffers().momentary + 976, 16).view(np.uint32).tolist()
             if best is None or kms < best[0]:
-                best = (kms, tms, ph, sub)
+                best = (kms, tms, ph, sub, ev)
                 hist = sim.memcpy_dtoh(sim.buffers().momentary + 1008, 12 * 32).view(np.uint64).reshape(12, 4)
-        kms, tms, ph, sub = best
+        kms, tms, ph, sub, ev = best
         vb = sim.memcpy_dtoh(sim.buffers().momentary + 64, 32).view(np.uint64)
         print("terrain %dM [%s]: kernel %.3f ms = %.0f Mpts/s, total %.3f ms = %.0f Mpts/s | voxels fresh/rewalk %d/%d spilled %d | nodes %d"
               % (K, "shipped" if module is None else "timers=2 build", kms, n / kms / 1e3, tms, n / tms / 1e3, int(vb[0]), int(vb[1]), int(vb[2]), st.numNodes), flush=True)
+        print("   events (legacy rounds, list-full warps, table-full counts, refused splits): %s" % ev, flush=True)
         if ph.sum() > 0:
             print("   us/batch %s | rounds/batch %.2f" % ({k: round(float(v) / 1e3 / K, 1) for k, v in zip(PHASES, ph) if k != "rounds(count)"}, ph[6] / K), flush=True)
             print("   block 0 timeline, us/batch:", {k: round(float(v) / 1e3 / K, 1) for k, v in zip(SUBS, sub)}, flush=True)
