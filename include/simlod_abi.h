@@ -169,6 +169,29 @@ typedef struct SimlodExportInfo {
     uint64_t num_samples, num_points, num_voxels;
 } SimlodExportInfo;
 
+// Header of an octree file (simlod_save_octree / simlod_load_octree), format version 1, little-endian. The file is this
+// 128-byte header, then `info.num_nodes` SimlodExportNode records (byte for byte the node table of the full export), then
+// one u32 Node::counter per record, then, at a 16-byte aligned offset, `info.num_samples` 16-byte samples (byte for byte
+// the full export's sample array). Reserved bytes are zero.
+#define SIMLOD_OCTREE_MAGIC "SIMLODOT"
+enum { SIMLOD_OCTREE_VERSION = 1, SIMLOD_OCTREE_HEADER_SIZE = 128 };
+typedef struct SimlodOctreeFileHeader {
+    char             magic[8];             //   0  "SIMLODOT", no terminator
+    uint32_t         version;              //   8  SIMLOD_OCTREE_VERSION
+    uint32_t         header_size;          //  12  SIMLOD_OCTREE_HEADER_SIZE
+    SimlodExportInfo info;                 //  16  the full export's counts and deepest level
+    float            box_min[3];           //  48  Uniforms::boxMin at save time
+    float            box_max[3];           //  60  Uniforms::boxMax at save time
+    uint32_t         batchlet_index;       //  72  Stats::batchletIndex
+    uint32_t         reserved0;            //  76
+    uint64_t         num_points_processed; //  80  Stats::numPointsProcessed
+    uint64_t         records_offset;       //  88  = header_size
+    uint64_t         counters_offset;      //  96  = records_offset + 64 * num_nodes
+    uint64_t         samples_offset;       // 104  = counters_offset + 4 * num_nodes, rounded up to 16
+    uint64_t         file_size;            // 112  = samples_offset + 16 * num_samples
+    uint64_t         reserved1;            // 120
+} SimlodOctreeFileHeader;
+
 // The LAS public header fields the reference reads (LasLoader.h:21-55), at their file byte offsets:
 typedef struct SimlodLasHeader {
     uint32_t version_major, version_minor;        // bytes 24, 25 (u8)
@@ -234,3 +257,16 @@ SIMLOD_STATIC_ASSERT(offsetof(SimlodLasHeader, scale) == 32, "LasHeader.scale");
 SIMLOD_STATIC_ASSERT(offsetof(SimlodLasHeader, min) == 80, "LasHeader.min");
 SIMLOD_STATIC_ASSERT(offsetof(SimlodLasHeader, max) == 104, "LasHeader.max");
 SIMLOD_STATIC_ASSERT(offsetof(SimlodExportInfo, num_samples) == 8, "ExportInfo.num_samples");
+SIMLOD_STATIC_ASSERT(sizeof(SimlodOctreeFileHeader) == 128, "OctreeFileHeader");
+SIMLOD_STATIC_ASSERT(offsetof(SimlodOctreeFileHeader, version) == 8, "OctreeFileHeader.version");
+SIMLOD_STATIC_ASSERT(offsetof(SimlodOctreeFileHeader, header_size) == 12, "OctreeFileHeader.header_size");
+SIMLOD_STATIC_ASSERT(offsetof(SimlodOctreeFileHeader, info) == 16, "OctreeFileHeader.info");
+SIMLOD_STATIC_ASSERT(offsetof(SimlodOctreeFileHeader, box_min) == 48, "OctreeFileHeader.box_min");
+SIMLOD_STATIC_ASSERT(offsetof(SimlodOctreeFileHeader, box_max) == 60, "OctreeFileHeader.box_max");
+SIMLOD_STATIC_ASSERT(offsetof(SimlodOctreeFileHeader, batchlet_index) == 72, "OctreeFileHeader.batchlet_index");
+SIMLOD_STATIC_ASSERT(offsetof(SimlodOctreeFileHeader, num_points_processed) == 80, "OctreeFileHeader.num_points_processed");
+SIMLOD_STATIC_ASSERT(offsetof(SimlodOctreeFileHeader, records_offset) == 88, "OctreeFileHeader.records_offset");
+SIMLOD_STATIC_ASSERT(offsetof(SimlodOctreeFileHeader, counters_offset) == 96, "OctreeFileHeader.counters_offset");
+SIMLOD_STATIC_ASSERT(offsetof(SimlodOctreeFileHeader, samples_offset) == 104, "OctreeFileHeader.samples_offset");
+SIMLOD_STATIC_ASSERT(offsetof(SimlodOctreeFileHeader, file_size) == 112, "OctreeFileHeader.file_size");
+SIMLOD_STATIC_ASSERT(offsetof(SimlodOctreeFileHeader, reserved1) == 120, "OctreeFileHeader.reserved1");

@@ -196,6 +196,31 @@ int simlod_export_octree(SimlodContext* ctx, int32_t depth, uint64_t dst_nodes, 
 int simlod_export_view(SimlodContext* ctx, uint64_t dst_nodes, uint64_t node_capacity, uint64_t dst_samples,
                        uint64_t sample_capacity, SimlodExportInfo* info, float* kernel_ms);
 
+// Octree files (SimlodOctreeFileHeader, DESIGN.md §9.7): a built octree saved and loaded back, so that it can be rendered,
+// exported or continued with new batches in another context, process or session.
+// simlod_read_octree_header: the header of an octree file, checked against itself and the file size. No context, no GPU.
+// SIMLOD_ERR_INVALID, naming the file, for a missing or short file, a wrong magic or version, or section offsets and sizes
+// that disagree with the header or the file size.
+int simlod_read_octree_header(const char* path, SimlodOctreeFileHeader* out);
+// Saves the octree as the last completed kernel_construct left it (batches still waiting in the ring are not part of it):
+// the full export's records and samples, the nodes' counters, the box and Stats::batchletIndex / numPointsProcessed.
+// Writes nothing into the context's buffers or Stats. SIMLOD_ERR_INVALID for an octree whose Stats::dbg has a bit other
+// than SIMLOD_DBG_FAR_POINT set, an inconsistent image, or a file that cannot be written. *info (optional) receives the
+// export's counts, *kernel_ms (optional) the event time of the export kernels. Staging memory is bounded (the file
+// streamer's page-locked pool and a 256 MB device window), whatever the octree's size.
+int simlod_save_octree(SimlodContext* ctx, const char* path, SimlodExportInfo* info, float* kernel_ms);
+// Replaces the context's octree by the file's (the counterpart of reload(), like simlod_insert_files): nodes[], heap,
+// Stats, the box of the uniforms (camera and settings stay), the ring counters and the builder's side tables, so that the
+// next kernel_construct launch continues as it would have in the context that saved the tree. Samples stream through
+// the page-locked pool, read by `loader_threads` threads. Errors name the file:
+//   SIMLOD_ERR_INVALID  bad header or records that are not a full export: nothing in the context is changed;
+//   SIMLOD_ERR_CAPACITY more records than nodes[] holds, more than 65 536 non-empty leaves, or a heap image that does not
+//                       fit the persistent buffer below the capacity guard's 200 MB margin: nothing is changed;
+//   SIMLOD_ERR_MODULE   a construct program other than the built-in one is loaded: nothing is changed;
+//   SIMLOD_ERR_INVALID  found while the samples are placed (a point outside its leaf, a voxel off its cell centre, two
+//                       voxels in one cell, a failed read): the context is left reset to an empty octree with the file's box.
+int simlod_load_octree(SimlodContext* ctx, const char* path, int loader_threads, SimlodExportInfo* info, float* kernel_ms);
+
 // Raw access for tests and tools: device addresses and sizes of the buffers the kernels share
 // (nodes[], persistent heap, momentary buffer, render buffer, point ring) and a bounded copy.
 typedef struct SimlodBuffers {

@@ -126,6 +126,14 @@ class ExportInfo(C.Structure):
                 ("num_voxels", C.c_uint64)]
 
 
+class OctreeFileHeader(C.Structure):
+    """SimlodOctreeFileHeader: the 128-byte header of an octree file (SimLOD.save_octree), format version 1."""
+    _fields_ = [("magic", C.c_char * 8), ("version", C.c_uint32), ("header_size", C.c_uint32), ("info", ExportInfo),
+                ("box_min", C.c_float * 3), ("box_max", C.c_float * 3), ("batchlet_index", C.c_uint32), ("reserved0", C.c_uint32),
+                ("num_points_processed", C.c_uint64), ("records_offset", C.c_uint64), ("counters_offset", C.c_uint64),
+                ("samples_offset", C.c_uint64), ("file_size", C.c_uint64), ("reserved1", C.c_uint64)]
+
+
 class OctreeExport:
     """SimLOD.export_octree() / export_view(): `nodes` (EXPORT_NODE_DTYPE records, breadth-first), `samples` (the sample
     array), `info`."""
@@ -137,6 +145,7 @@ class OctreeExport:
 assert C.sizeof(Uniforms) == 480 and C.sizeof(Stats) == 112
 assert C.sizeof(ExportInfo) == 32 and EXPORT_NODE_DTYPE.itemsize == 64
 assert C.sizeof(LasHeader) == 128
+assert C.sizeof(OctreeFileHeader) == 128
 
 # every symbol include/simlod_b200.h declares
 EXPORTS = [
@@ -149,6 +158,7 @@ EXPORTS = [
     "simlod_partition_count", "simlod_partition_scatter", "simlod_partition_wait",
     "simlod_export_framebuffer", "simlod_peer_signal", "simlod_composite_framebuffers", "simlod_generate", "simlod_reset_with_grid", "simlod_insert_simlod_file_ex", "simlod_get_numa_node",
     "simlod_export_octree", "simlod_export_view", "simlod_read_las_header", "simlod_insert_files",
+    "simlod_read_octree_header", "simlod_save_octree", "simlod_load_octree",
 ]
 
 _lib = None
@@ -208,6 +218,9 @@ def load_library():
         "simlod_export_view": [vp, u64, u64, u64, u64, C.POINTER(ExportInfo), C.POINTER(C.c_float)],
         "simlod_read_las_header": [C.c_char_p, C.POINTER(LasHeader)],
         "simlod_insert_files": [vp, C.POINTER(C.c_char_p), u32, C.c_int, u32, C.POINTER(u64), C.POINTER(C.c_float), C.POINTER(C.c_float)],
+        "simlod_read_octree_header": [C.c_char_p, C.POINTER(OctreeFileHeader)],
+        "simlod_save_octree": [vp, C.c_char_p, C.POINTER(ExportInfo), C.POINTER(C.c_float)],
+        "simlod_load_octree": [vp, C.c_char_p, C.c_int, C.POINTER(ExportInfo), C.POINTER(C.c_float)],
     }
     for name, argtypes in sig.items():
         fn = getattr(lib, name)
@@ -223,6 +236,17 @@ def read_las_header(path):
     lib = load_library()
     h = LasHeader()
     rc = lib.simlod_read_las_header(os.fsencode(path), C.byref(h))
+    if rc != 0:
+        raise SimlodError(rc, lib.simlod_last_error().decode())
+    return h
+
+
+def read_octree_header(path):
+    """The header of an octree file (simlod_read_octree_header), checked against itself and the file size: an
+    OctreeFileHeader. Needs no GPU. Raises SimlodError(-2) naming the file when it is not a valid octree file."""
+    lib = load_library()
+    h = OctreeFileHeader()
+    rc = lib.simlod_read_octree_header(os.fsencode(path), C.byref(h))
     if rc != 0:
         raise SimlodError(rc, lib.simlod_last_error().decode())
     return h
@@ -414,6 +438,24 @@ class SimLOD:
         self._lib.simlod_get_uniforms(self._ctx, C.byref(self.uniforms))
         self._check(rc)
         return n.value, kms.value, tms.value
+
+    def save_octree(self, path):
+        """Save the octree, as the last completed update left it, to an octree file (simlod_save_octree): the full
+        export's records and samples (np.memmap-able at the header's offsets), the nodes' counters, the box and the batch
+        counters. Writes nothing into the context. Returns (ExportInfo, kernel ms)."""
+        info, ms = ExportInfo(), C.c_float(0)
+        self._check(self._lib.simlod_save_octree(self._ctx, os.fsencode(path), C.byref(info), C.byref(ms)))
+        return info, ms.value
+
+    def load_octree(self, path, loader_threads=16):
+        """Replace the octree by an octree file's (simlod_load_octree): render it, export it or insert further batches,
+        which continue as they would have in the context that saved it. Sets the box of the uniforms; the camera and
+        settings stay. Returns (ExportInfo, kernel ms)."""
+        info, ms = ExportInfo(), C.c_float(0)
+        rc = self._lib.simlod_load_octree(self._ctx, os.fsencode(path), int(loader_threads), C.byref(info), C.byref(ms))
+        self._lib.simlod_get_uniforms(self._ctx, C.byref(self.uniforms))
+        self._check(rc)
+        return info, ms.value
 
     def insert_batches(self, batches):
         """Insert explicit batches (each <= 1 M points), each followed by update launches until the

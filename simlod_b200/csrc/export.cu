@@ -18,6 +18,10 @@
 //   simlod_export_gather   after the host has checked ExportCtl: warps copy the node records, then pop chunk items
 //                          (<= 1000 samples each) and copy them with 16-byte loads and coalesced streaming stores
 //
+// The octree file (simlod_save_octree, DESIGN.md §9.7) runs the full plan and collect, then simlod_export_counters (the
+// records' Node::counter) and simlod_export_gather_window, the gather's instance that copies one bounded window of the
+// sample array at a time.
+//
 // The flags, plan and collect kernels write scratch and ExportCtl only; nothing reaches the destination before the
 // gather. Nothing is written into nodes[] (not even the visible / isLarge flags kernel_render stores there).
 #include <stdint.h>
@@ -316,21 +320,34 @@ simlod_export_collect(const uint8_t* __restrict__ nodes, const uint8_t* __restri
 
 constexpr uint32_t GATHER_UNROLL = 8;
 
-extern "C" __global__ void __launch_bounds__(256)
-simlod_export_gather(const uint4* __restrict__ rec, uint4* __restrict__ dstNodes, const Item* __restrict__ items,
-                     uint4* __restrict__ dstSamples, const ExportCtl* __restrict__ ctl) {
+// windowed: the octree file's staging (simlod_save_octree) — no records, and of every item only the samples whose
+// destination index lies in [winBegin, winEnd), written at index - winBegin. A template parameter, so that the export's
+// own gather compiles to the kernel it was before the window existed.
+template <bool windowed>
+__device__ __forceinline__ void gather(const uint4* __restrict__ rec, uint4* __restrict__ dstNodes, const Item* __restrict__ items,
+                                       uint4* __restrict__ dstSamples, const ExportCtl* __restrict__ ctl, uint64_t winBegin, uint64_t winEnd) {
     const uint32_t lane = threadIdx.x & 31u;
     const uint64_t warp = ((uint64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
     const uint64_t numWarps = ((uint64_t)gridDim.x * blockDim.x) >> 5;
-    const uint64_t recWords = (uint64_t)ctl->numNodes * (sizeof(SimlodExportNode) / 16);
-    for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < recWords; i += (uint64_t)gridDim.x * blockDim.x)
-        __stcs(dstNodes + i, rec[i]);
+    if (!windowed) {
+        const uint64_t recWords = (uint64_t)ctl->numNodes * (sizeof(SimlodExportNode) / 16);
+        for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < recWords; i += (uint64_t)gridDim.x * blockDim.x)
+            __stcs(dstNodes + i, rec[i]);
+    }
     const uint64_t numItems = ctl->numItems;
     for (uint64_t k = warp; k < numItems; k += numWarps) {
         const Item it = items[k];
         const uint4* __restrict__ src = (const uint4*)it.src;
         uint4* __restrict__ dst = dstSamples + (it.dst & 0xffffffffffffull);
-        const uint32_t count = (uint32_t)(it.dst >> 48);
+        uint32_t count = (uint32_t)(it.dst >> 48);
+        if (windowed) {
+            const uint64_t d0 = it.dst & 0xffffffffffffull;
+            const uint64_t lo = max(d0, winBegin), hi = min(d0 + count, winEnd);
+            if (lo >= hi) continue;
+            src += lo - d0;
+            dst = dstSamples + (lo - winBegin);
+            count = (uint32_t)(hi - lo);
+        }
         for (uint32_t b = 0; b < count; b += 32 * GATHER_UNROLL) {
             uint4 v[GATHER_UNROLL];
             #pragma unroll
@@ -345,4 +362,25 @@ simlod_export_gather(const uint4* __restrict__ rec, uint4* __restrict__ dstNodes
             }
         }
     }
+}
+
+extern "C" __global__ void __launch_bounds__(256)
+simlod_export_gather(const uint4* __restrict__ rec, uint4* __restrict__ dstNodes, const Item* __restrict__ items,
+                     uint4* __restrict__ dstSamples, const ExportCtl* __restrict__ ctl) {
+    gather<false>(rec, dstNodes, items, dstSamples, ctl, 0, 0);
+}
+
+// The samples of the full export whose index lies in [winBegin, winEnd), into window[0, winEnd - winBegin)
+extern "C" __global__ void __launch_bounds__(256)
+simlod_export_gather_window(const Item* __restrict__ items, uint4* __restrict__ window, const ExportCtl* __restrict__ ctl,
+                            uint64_t winBegin, uint64_t winEnd) {
+    gather<true>(nullptr, nullptr, items, window, ctl, winBegin, winEnd);
+}
+
+// Node::counter of every record's node (the octree file's counters section; the records do not carry it)
+extern "C" __global__ void __launch_bounds__(256)
+simlod_export_counters(const SimlodNode* __restrict__ nodes, const uint32_t* __restrict__ recNode, const ExportCtl* __restrict__ ctl,
+                       uint32_t* __restrict__ counters) {
+    const uint32_t n = ctl->numNodes;
+    for (uint32_t r = blockIdx.x * blockDim.x + threadIdx.x; r < n; r += gridDim.x * blockDim.x) counters[r] = nodes[recNode[r]].counter;
 }

@@ -45,6 +45,7 @@ extern const unsigned char simlod_cubin_partition[];
 extern const unsigned char simlod_cubin_las[];
 extern const unsigned char simlod_cubin_gen[];
 extern const unsigned char simlod_cubin_export[];
+extern const unsigned char simlod_cubin_import[];
 }
 
 namespace {
@@ -112,6 +113,7 @@ struct Program {
 }  // namespace
 
 #include "loader_pool.h"
+#include "construct_layout.cuh"
 
 struct SimlodContext {
     CUdevice device = 0;
@@ -168,6 +170,13 @@ struct SimlodContext {
     CUdeviceptr exportScratch = 0;     // octree export: records | node indices | first items | chunk items | ExportCtl
     uint64_t exportScratchBytes = 0;
     void* hExportCtl = nullptr;        // pinned copy of ExportCtl
+    CUfunction fnExportGatherWindow = nullptr, fnExportCounters = nullptr;
+    CUmodule importModule = nullptr;
+    CUfunction fnImportNodes = nullptr, fnImportLink = nullptr, fnImportClearGrids = nullptr, fnImportScatter = nullptr,
+               fnImportVoxels = nullptr, fnImportCountGrids = nullptr;
+    CUdeviceptr fileWindow = 0;        // octree files: FILE_WINDOW_BYTES of samples staged on the device
+    CUdeviceptr fileTables = 0;        // octree load: records | plan | error word, sized for nodes[]
+    uint64_t fileTablesBytes = 0;
     void* pinnedPool = nullptr;        // POOL_BYTES page-locked: the file streamer's slots, one batch of records each
     LoaderPool* loaderPool = nullptr;
     CUevent evPool[32] = {};           // H2D copy out of pool slot i has been enqueued and completed
@@ -459,6 +468,15 @@ static int createResources(SimlodContext* ctx, const SimlodConfig* config) {
     CU(D(cuModuleGetFunction)(&ctx->fnExportGather, ctx->exportModule, "simlod_export_gather"));
     CU(D(cuModuleGetFunction)(&ctx->fnExportViewFlags, ctx->exportModule, "simlod_export_view_flags"));
     CU(D(cuModuleGetFunction)(&ctx->fnExportPlanView, ctx->exportModule, "simlod_export_plan_view"));
+    CU(D(cuModuleGetFunction)(&ctx->fnExportGatherWindow, ctx->exportModule, "simlod_export_gather_window"));
+    CU(D(cuModuleGetFunction)(&ctx->fnExportCounters, ctx->exportModule, "simlod_export_counters"));
+    CU(D(cuModuleLoadData)(&ctx->importModule, simlod_cubin_import));
+    CU(D(cuModuleGetFunction)(&ctx->fnImportNodes, ctx->importModule, "simlod_import_nodes"));
+    CU(D(cuModuleGetFunction)(&ctx->fnImportLink, ctx->importModule, "simlod_import_link"));
+    CU(D(cuModuleGetFunction)(&ctx->fnImportClearGrids, ctx->importModule, "simlod_import_clear_grids"));
+    CU(D(cuModuleGetFunction)(&ctx->fnImportScatter, ctx->importModule, "simlod_import_scatter"));
+    CU(D(cuModuleGetFunction)(&ctx->fnImportVoxels, ctx->importModule, "simlod_import_voxels"));
+    CU(D(cuModuleGetFunction)(&ctx->fnImportCountGrids, ctx->importModule, "simlod_import_count_grids"));
 
     // buffers (main.cpp:552-586)
     SimlodBuffers& b = ctx->buf;
@@ -569,6 +587,9 @@ void simlod_destroy(SimlodContext* ctx) {
         if (ctx->exportModule) D(cuModuleUnload)(ctx->exportModule);
         if (ctx->exportScratch) D(cuMemFree)(ctx->exportScratch);
         if (ctx->hExportCtl) D(cuMemFreeHost)(ctx->hExportCtl);
+        if (ctx->importModule) D(cuModuleUnload)(ctx->importModule);
+        if (ctx->fileWindow) D(cuMemFree)(ctx->fileWindow);
+        if (ctx->fileTables) D(cuMemFree)(ctx->fileTables);
         delete ctx->loaderPool;          // joins the loader threads
         if (ctx->pinnedPool) D(cuMemFreeHost)(ctx->pinnedPool);
         for (int i = 0; i < 32; i++) if (ctx->evPool[i]) D(cuEventDestroy)(ctx->evPool[i]);
@@ -1005,6 +1026,15 @@ int probeLas(const char* path, StreamFile* out) {
     return SIMLOD_OK;
 }
 
+// the streamer's page-locked pool (POOL_BYTES) and its slot events, allocated on first use
+int ensurePinnedPool(SimlodContext* ctx) {
+    if (ctx->pinnedPool) return SIMLOD_OK;
+    NumaLocal onGpuNode(ctx);
+    CU(D(cuMemHostAlloc)(&ctx->pinnedPool, (size_t)POOL_BYTES, CU_MEMHOSTALLOC_PORTABLE));
+    for (uint64_t i = 0; i < MAX_POOL_SLOTS; i++) CU(D(cuEventCreate)(&ctx->evPool[i], CU_EVENT_DISABLE_TIMING));
+    return SIMLOD_OK;
+}
+
 int openForStream(StreamFile* f, bool direct) {
     // SIMLOD_STREAM_DIRECT: unbuffered reads, as the reference's Windows loader does (SimlodLoader.cpp:59-141, FILE_FLAG_NO_BUFFERING):
     // whole 4 KB blocks straight from the device into a per-thread block buffer — no page-cache copy, no cache pollution —
@@ -1043,11 +1073,7 @@ static int streamFiles(SimlodContext* ctx, StreamFiles& files, int loader_thread
     if (num_points) *num_points = numPoints;
     for (int i = 0; i < 3; i++) { ctx->uniforms.boxMin[i] = 0.0f; ctx->uniforms.boxMax[i] = bmax[i] - bmin[i]; }   // main.cpp:312-313
     int rc = simlod_reset(ctx); if (rc) return rc;                        // reload() -> reset
-    if (!ctx->pinnedPool) {
-        NumaLocal onGpuNode(ctx);
-        CU(D(cuMemHostAlloc)(&ctx->pinnedPool, (size_t)POOL_BYTES, CU_MEMHOSTALLOC_PORTABLE));
-        for (uint64_t i = 0; i < MAX_POOL_SLOTS; i++) CU(D(cuEventCreate)(&ctx->evPool[i], CU_EVENT_DISABLE_TIMING));
-    }
+    rc = ensurePinnedPool(ctx); if (rc) return rc;
     if (maxLasBpp) { rc = ensureStaging(ctx, SLOT_POINTS * maxLasBpp); if (rc) return rc; }
     // a pool slot holds one batch of the largest records in the list: 32 slots of 16 MB for .simlod points, 5 of 96 MB
     // for the largest LAS records. SLOT_POINTS * bpp is a multiple of 16, so every slot and piece starts 16-byte aligned.
@@ -1388,13 +1414,14 @@ struct ExportViewScratch {           // mirrors export.cu ViewScratch
 };
 constexpr uint64_t align16(uint64_t v) { return (v + 15) & ~15ull; }
 
-// The export of simlod_export_octree (view == nullptr) and simlod_export_view (the LOD cut for *view).
-int exportOctree(SimlodContext* ctx, int32_t depth, const SimlodUniforms* view, uint64_t dst_nodes, uint64_t node_capacity,
-                 uint64_t dst_samples, uint64_t sample_capacity, SimlodExportInfo* info, float* kernel_ms) {
-    int rc = setCurrent(ctx); if (rc) return rc;
-    if (!info) return fail(SIMLOD_ERR_INVALID, "null info");
-    if (depth > SIMLOD_MAX_DEPTH) return fail(SIMLOD_ERR_INVALID, "export depth %d exceeds the octree's maximum depth %d", depth, (int)SIMLOD_MAX_DEPTH);
-    if (dst_nodes % 16 || dst_samples % 16) return fail(SIMLOD_ERR_INVALID, "export destinations must be 16-byte aligned");
+// Stage 1 of an export, into scratch only: the view's drawn flags, the plan and the chunk-list walk. On success p holds
+// the checked ExportCtl and where the records, node indices, chunk items and ExportCtl lie.
+struct ExportPlanned {
+    CUdeviceptr rec = 0, recNode = 0, items = 0, ctl = 0;
+    ExportCtl c{};
+    float ms = 0.0f;
+};
+int exportPlan(SimlodContext* ctx, int32_t depth, const SimlodUniforms* view, ExportPlanned* p) {
     // scratch, sized by the context's buffers: one record per node of nodes[], one item per chunk the heap can hold; the
     // view adds per node a drawn byte, and per record a mark byte, an index and a second record and node index
     const uint32_t maxRecords = (uint32_t)(ctx->buf.nodes_bytes / sizeof(SimlodNode));
@@ -1444,9 +1471,26 @@ int exportOctree(SimlodContext* ctx, int32_t depth, const SimlodUniforms* view, 
     const ExportCtl c = *(const ExportCtl*)ctx->hExportCtl;
     float ms = 0.0f;
     CU(D(cuEventElapsedTime)(&ms, ctx->evStart, ctx->evEnd));
-    if (kernel_ms) *kernel_ms = ms;
+    p->rec = rec; p->recNode = recNode; p->items = items; p->ctl = ctl; p->c = c; p->ms = ms;
     if (c.error)
         return fail(SIMLOD_ERR_INVALID, "octree image is inconsistent (error %u: 1 child pointer outside nodes[], 2 chunk pointer outside the used heap, 4 list shorter than its count, 5 inner node without 8 children)", c.error);
+    return SIMLOD_OK;
+}
+
+// The export of simlod_export_octree (view == nullptr) and simlod_export_view (the LOD cut for *view).
+int exportOctree(SimlodContext* ctx, int32_t depth, const SimlodUniforms* view, uint64_t dst_nodes, uint64_t node_capacity,
+                 uint64_t dst_samples, uint64_t sample_capacity, SimlodExportInfo* info, float* kernel_ms) {
+    int rc = setCurrent(ctx); if (rc) return rc;
+    if (!info) return fail(SIMLOD_ERR_INVALID, "null info");
+    if (depth > SIMLOD_MAX_DEPTH) return fail(SIMLOD_ERR_INVALID, "export depth %d exceeds the octree's maximum depth %d", depth, (int)SIMLOD_MAX_DEPTH);
+    if (dst_nodes % 16 || dst_samples % 16) return fail(SIMLOD_ERR_INVALID, "export destinations must be 16-byte aligned");
+    ExportPlanned p;
+    rc = exportPlan(ctx, depth, view, &p);
+    if (kernel_ms) *kernel_ms = p.ms;
+    if (rc) return rc;
+    const ExportCtl c = p.c;
+    const float ms = p.ms;
+    CUdeviceptr rec = p.rec, items = p.items, ctl = p.ctl;
     info->num_nodes = c.numNodes; info->max_level = c.maxLevel;
     info->num_samples = c.numSamples; info->num_points = c.numPoints; info->num_voxels = c.numVoxels;
     if (!dst_nodes && !dst_samples) return SIMLOD_OK;          // size query
@@ -1478,6 +1522,428 @@ int simlod_export_view(SimlodContext* ctx, uint64_t dst_nodes, uint64_t node_cap
                        uint64_t sample_capacity, SimlodExportInfo* info, float* kernel_ms) {
     if (!ctx) return fail(SIMLOD_ERR_INVALID, "null context");
     return exportOctree(ctx, -1, &ctx->uniforms, dst_nodes, node_capacity, dst_samples, sample_capacity, info, kernel_ms);
+}
+
+// ---- octree files (DESIGN.md §9.7); kernels in export.cu (save) and import.cu (load) ---------------------------------
+}  // extern "C"
+
+namespace {
+constexpr uint64_t FILE_WINDOW_BYTES = POOL_BYTES / 2;             // samples per staged window: half the page-locked pool
+constexpr uint64_t FILE_WINDOW_SAMPLES = FILE_WINDOW_BYTES / sizeof(SimlodPoint);
+constexpr uint64_t HEAP_GUARD_BYTES = 200000000ull;                // kernel_construct's capacity guard (construct.cu)
+constexpr uint32_t NODE_TABLE_CAP = (uint32_t)scratch::NODE_CAP;  // the builder's side tables
+constexpr uint32_t ROW_CAP = (uint32_t)scratch::ROW_CAP, ROW_SLOTS = (uint32_t)scratch::ROW_SLOTS;   // chunk rows
+
+struct ImportPlan { uint64_t grid; uint64_t chunk; uint32_t row; uint32_t counter; };   // mirrors import.cu
+struct ImportArgs {                                                                         // mirrors import.cu
+    CUdeviceptr nodes, heap, scratch, rec, plan, error;
+    uint64_t chunkBase;
+    uint32_t numRecords, numRows;
+    float boxMin[3], boxMax[3];
+};
+static_assert(sizeof(ImportPlan) == 24 && sizeof(ImportArgs) == 88, "import.cu layouts");
+
+// where each section of a file with n records and s samples lies (SimlodOctreeFileHeader)
+void octreeLayout(uint64_t n, uint64_t s, SimlodOctreeFileHeader* h) {
+    h->records_offset = SIMLOD_OCTREE_HEADER_SIZE;
+    h->counters_offset = h->records_offset + n * sizeof(SimlodExportNode);
+    h->samples_offset = align16(h->counters_offset + 4 * n);
+    h->file_size = h->samples_offset + s * sizeof(SimlodPoint);
+}
+
+int readOctreeHeader(const char* path, SimlodOctreeFileHeader* out) {
+    struct stat st;
+    if (stat(path, &st) != 0) return fail(SIMLOD_ERR_INVALID, "cannot open %s", path);
+    FILE* f = fopen(path, "rb");
+    if (!f) return fail(SIMLOD_ERR_INVALID, "cannot open %s", path);
+    SimlodOctreeFileHeader h;
+    const size_t got = fread(&h, 1, sizeof(h), f);
+    fclose(f);
+    if (got != sizeof(h)) return fail(SIMLOD_ERR_INVALID, "%s is shorter than an octree file header (%zu bytes)", path, got);
+    if (memcmp(h.magic, SIMLOD_OCTREE_MAGIC, 8) != 0) return fail(SIMLOD_ERR_INVALID, "%s is not an octree file (no SIMLODOT magic)", path);
+    if (h.version != SIMLOD_OCTREE_VERSION) return fail(SIMLOD_ERR_INVALID, "%s: octree file version %u, this library reads version %d", path, h.version, (int)SIMLOD_OCTREE_VERSION);
+    if (h.header_size != SIMLOD_OCTREE_HEADER_SIZE) return fail(SIMLOD_ERR_INVALID, "%s: header size %u, expected %d", path, h.header_size, (int)SIMLOD_OCTREE_HEADER_SIZE);
+    if (h.info.num_nodes == 0 || h.info.num_points + h.info.num_voxels != h.info.num_samples || h.info.num_samples < h.info.num_points ||
+        h.info.num_samples > (std::numeric_limits<uint64_t>::max() >> 5) || h.info.max_level > SIMLOD_MAX_DEPTH || h.reserved0 || h.reserved1)
+        return fail(SIMLOD_ERR_INVALID, "%s: inconsistent header (%u records, %llu samples = %llu points + %llu voxels, deepest level %u)", path,
+                    h.info.num_nodes, (unsigned long long)h.info.num_samples, (unsigned long long)h.info.num_points, (unsigned long long)h.info.num_voxels, h.info.max_level);
+    SimlodOctreeFileHeader want = h;
+    octreeLayout(h.info.num_nodes, h.info.num_samples, &want);
+    if (h.records_offset != want.records_offset || h.counters_offset != want.counters_offset || h.samples_offset != want.samples_offset ||
+        h.file_size != want.file_size)
+        return fail(SIMLOD_ERR_INVALID, "%s: section offsets (%llu, %llu, %llu, size %llu) disagree with %u records and %llu samples", path,
+                    (unsigned long long)h.records_offset, (unsigned long long)h.counters_offset, (unsigned long long)h.samples_offset,
+                    (unsigned long long)h.file_size, h.info.num_nodes, (unsigned long long)h.info.num_samples);
+    if ((uint64_t)st.st_size != h.file_size)
+        return fail(SIMLOD_ERR_INVALID, "%s is %llu bytes, its header describes %llu", path, (unsigned long long)st.st_size, (unsigned long long)h.file_size);
+    *out = h;
+    return SIMLOD_OK;
+}
+
+int ensureFileWindow(SimlodContext* ctx) {
+    if (!ctx->fileWindow) CU(D(cuMemAlloc)(&ctx->fileWindow, FILE_WINDOW_BYTES));
+    return ensurePinnedPool(ctx);
+}
+
+bool writeAll(FILE* f, const void* p, uint64_t bytes) { return bytes == 0 || fwrite(p, 1, bytes, f) == bytes; }
+
+int saveOctree(SimlodContext* ctx, const char* path, SimlodExportInfo* info, float* kernel_ms) {
+    int rc = setCurrent(ctx); if (rc) return rc;
+    if (!path) return fail(SIMLOD_ERR_INVALID, "null path");
+    // the octree as the last completed launch left it
+    CU(D(cuStreamSynchronize)(ctx->streamCopy));
+    CU(D(cuStreamSynchronize)(ctx->streamUpload));
+    rc = readStats(ctx); if (rc) return rc;
+    const SimlodStats st = *ctx->hStats;
+    if (st.dbg & ~(uint32_t)SIMLOD_DBG_FAR_POINT)
+        return fail(SIMLOD_ERR_INVALID, "%s: not saved, the octree's Stats::dbg is 0x%x (a capacity of the builder was exceeded)", path, st.dbg);
+    ExportPlanned p;
+    rc = exportPlan(ctx, -1, nullptr, &p);
+    if (rc) return fail(rc, "%s: not saved: %s", path, g_error.c_str());
+    rc = ensureFileWindow(ctx); if (rc) return rc;
+    float ms = p.ms;
+    const uint32_t n = p.c.numNodes;
+    const uint64_t numSamples = p.c.numSamples;
+    SimlodOctreeFileHeader h;
+    memset(&h, 0, sizeof(h));
+    memcpy(h.magic, SIMLOD_OCTREE_MAGIC, 8);
+    h.version = SIMLOD_OCTREE_VERSION;
+    h.header_size = SIMLOD_OCTREE_HEADER_SIZE;
+    h.info.num_nodes = n; h.info.max_level = p.c.maxLevel;
+    h.info.num_samples = numSamples; h.info.num_points = p.c.numPoints; h.info.num_voxels = p.c.numVoxels;
+    for (int i = 0; i < 3; i++) { h.box_min[i] = ctx->uniforms.boxMin[i]; h.box_max[i] = ctx->uniforms.boxMax[i]; }
+    h.batchlet_index = st.batchletIndex;
+    h.num_points_processed = st.numPointsProcessed;
+    octreeLayout(n, numSamples, &h);
+    // records and counters: bounded by nodes[]
+    std::vector<uint8_t> head(h.samples_offset, 0);
+    memcpy(head.data(), &h, sizeof(h));
+    CU(D(cuMemcpyDtoH)(head.data() + h.records_offset, p.rec, (size_t)n * sizeof(SimlodExportNode)));
+    CUdeviceptr nodes = ctx->buf.nodes, window = ctx->fileWindow, recNode = p.recNode, items = p.items, ctl = p.ctl;
+    SimlodContext::LaunchQueue& q = ctx->queue;
+    CU(D(cuEventRecord)(q.ev[0][0], ctx->streamMain));
+    { void* args[] = {&nodes, &recNode, &ctl, &window};
+      CU(D(cuLaunchKernel)(ctx->fnExportCounters, (unsigned)ctx->numSMs * 2, 1, 1, 256, 1, 1, 0, ctx->streamMain, args, nullptr)); }
+    CU(D(cuEventRecord)(q.ev[0][1], ctx->streamMain));
+    ctx->launches++;
+    CU(D(cuMemcpyDtoHAsync)(head.data() + h.counters_offset, window, (size_t)n * 4, ctx->streamMain));
+    CU(D(cuStreamSynchronize)(ctx->streamMain));
+    float t = 0.0f;
+    CU(D(cuEventElapsedTime)(&t, q.ev[0][0], q.ev[0][1]));
+    ms += t;
+    // written under a temporary name and renamed once complete: a failed save leaves no partial file and replaces
+    // no existing one
+    const std::string tmpPath = std::string(path) + ".tmp";
+    FILE* f = fopen(tmpPath.c_str(), "wb");
+    if (!f) return fail(SIMLOD_ERR_INVALID, "cannot write %s", path);
+    struct Closer {
+        FILE*& f; const std::string& tmp; bool done = false;
+        ~Closer() { if (f) fclose(f); if (!done) unlink(tmp.c_str()); }
+    } closer{f, tmpPath};
+    if (!writeAll(f, head.data(), head.size())) return fail(SIMLOD_ERR_INVALID, "write error in %s", path);
+    // samples: window w is gathered on the device and copied into pool half w & 1 while window w - 1 is written out
+    const uint64_t numWindows = (numSamples + FILE_WINDOW_SAMPLES - 1) / FILE_WINDOW_SAMPLES;
+    auto half = [&](uint64_t w) { return (char*)ctx->pinnedPool + (w & 1) * FILE_WINDOW_BYTES; };
+    auto windowSamples = [&](uint64_t w) { return std::min<uint64_t>(FILE_WINDOW_SAMPLES, numSamples - w * FILE_WINDOW_SAMPLES); };
+    auto drain = [&](uint64_t w) -> int {            // window w has been copied out: time it and write it
+        CU(D(cuEventSynchronize)(q.statsDone[w & 1]));
+        float g = 0.0f;
+        CU(D(cuEventElapsedTime)(&g, q.ev[w & 1][0], q.ev[w & 1][1]));
+        ms += g;
+        if (!writeAll(f, half(w), windowSamples(w) * sizeof(SimlodPoint))) return fail(SIMLOD_ERR_INVALID, "write error in %s", path);
+        return SIMLOD_OK;
+    };
+    for (uint64_t w = 0; w < numWindows; w++) {
+        uint64_t a = w * FILE_WINDOW_SAMPLES, b = a + windowSamples(w);
+        CU(D(cuEventRecord)(q.ev[w & 1][0], ctx->streamMain));
+        { void* args[] = {&items, &window, &ctl, &a, &b};
+          CU(D(cuLaunchKernel)(ctx->fnExportGatherWindow, (unsigned)ctx->numSMs * 4, 1, 1, 256, 1, 1, 0, ctx->streamMain, args, nullptr)); }
+        CU(D(cuEventRecord)(q.ev[w & 1][1], ctx->streamMain));
+        ctx->launches++;
+        CU(D(cuMemcpyDtoHAsync)(half(w), window, (size_t)(b - a) * sizeof(SimlodPoint), ctx->streamMain));
+        CU(D(cuEventRecord)(q.statsDone[w & 1], ctx->streamMain));
+        if (w > 0) { rc = drain(w - 1); if (rc) return rc; }
+    }
+    if (numWindows > 0) { rc = drain(numWindows - 1); if (rc) return rc; }
+    const int closed = fclose(f);
+    f = nullptr;
+    if (closed != 0) return fail(SIMLOD_ERR_INVALID, "write error in %s", path);
+    if (rename(tmpPath.c_str(), path) != 0) return fail(SIMLOD_ERR_INVALID, "cannot write %s (rename from %s failed)", path, tmpPath.c_str());
+    closer.done = true;
+    if (info) *info = h.info;
+    if (kernel_ms) *kernel_ms = ms;
+    return SIMLOD_OK;
+}
+
+// What load needs to know about a file's records beyond the records themselves: the heap plan and the Stats sweep.
+struct LoadPlan {
+    std::vector<ImportPlan> plan;      // one per record, then one with chunk = the total
+    uint64_t gridBase = 0, chunkBase = 0, heapEnd = 0, numChunks = 0;
+    uint32_t numGrids = 0, numRows = 0;
+    SimlodStats stats{};               // the sweep fields
+};
+
+// The checks that make the records a full export of a builder's octree (simlod_load_octree), and the heap plan.
+int planLoad(const char* path, const SimlodOctreeFileHeader& h, const SimlodExportNode* rec, const uint32_t* counters, LoadPlan* out) {
+    const uint32_t n = h.info.num_nodes;
+    auto bad = [&](uint32_t i, const char* what) { return fail(SIMLOD_ERR_INVALID, "%s: record %u: %s (not a full export of an octree)", path, i, what); };
+    std::vector<ImportPlan>& plan = out->plan;
+    plan.assign((size_t)n + 1, ImportPlan{0, 0, 0, 0});
+    static const uint8_t rootName[20] = {'r'};
+    if (rec[0].level != 0 || rec[0].X || rec[0].Y || rec[0].Z || rec[0].parent != -1 || memcmp(rec[0].name, rootName, 20) != 0) return bad(0, "not the root");
+    uint32_t next = 1, maxLevel = 0, innerNonRoot = 0;
+    uint64_t samples = 0, points = 0, voxels = 0, chunks = 0;
+    SimlodStats& s = out->stats;
+    for (uint32_t i = 0; i < n; i++) {
+        const SimlodExportNode& r = rec[i];
+        const bool inner = r.first_child >= 0;
+        if (r.level > SIMLOD_MAX_DEPTH) return bad(i, "level above 20");
+        if (r.first_child < -1) return bad(i, "bad first_child");
+        if (r.flags != ((uint32_t)SIMLOD_EXPORT_SAMPLED | (inner ? 0u : (uint32_t)SIMLOD_EXPORT_LEAF))) return bad(i, "flags other than SAMPLED, and LEAF exactly on childless records");
+        if (r.sample_offset != samples) return bad(i, "sample_offset is not the running sum");
+        if (inner && r.num_points) return bad(i, "points on an inner node");
+        if (!inner && i != 0 && r.num_voxels) return bad(i, "voxels on a leaf other than the root");
+        if (!inner && counters[i] != r.num_points) return bad(i, "a leaf's counter differs from its point count");
+        if (inner && counters[i] <= SIMLOD_MAX_POINTS_PER_NODE) return bad(i, "an inner node's counter is not above 50 000");
+        if (!inner && r.level < SIMLOD_MAX_DEPTH && r.num_points > SIMLOD_MAX_POINTS_PER_NODE) return bad(i, "a leaf above level 20 holds more than 50 000 points");
+        if (inner) {
+            // children: the next 8 records, in child-index order, one level down (breadth-first order follows)
+            if ((uint32_t)r.first_child != next || (uint64_t)next + 8 > n) return bad(i, "first_child is not the next 8 records in breadth-first order");
+            for (uint32_t k = 0; k < 8; k++) {
+                const SimlodExportNode& c = rec[next + k];
+                uint8_t name[20];
+                memcpy(name, r.name, 20);
+                if (r.level + 1 < 20) name[r.level + 1] = (uint8_t)('0' + k);
+                if (c.parent != (int32_t)i || c.level != r.level + 1 || c.X != 2 * r.X + ((k >> 2) & 1) || c.Y != 2 * r.Y + ((k >> 1) & 1) ||
+                    c.Z != 2 * r.Z + (k & 1) || memcmp(c.name, name, 20) != 0)
+                    return bad(next + k, "not the child of its parent (parent, level, X, Y, Z or name)");
+            }
+            next += 8;
+            s.numInner++;
+            s.numVoxels += r.num_voxels;
+            s.numChunksVoxels += (r.num_voxels + SIMLOD_POINTS_PER_CHUNK - 1) / SIMLOD_POINTS_PER_CHUNK;
+        } else {
+            s.numLeaves++;
+            s.numPoints += r.num_points;
+            s.numChunksPoints += (r.num_points + SIMLOD_POINTS_PER_CHUNK - 1) / SIMLOD_POINTS_PER_CHUNK;
+            if (r.num_points) s.numNonemptyLeaves++;
+        }
+        maxLevel = std::max(maxLevel, r.level);
+        samples += (uint64_t)r.num_points + r.num_voxels;
+        points += r.num_points;
+        voxels += r.num_voxels;
+        const uint32_t npc = (r.num_points + SIMLOD_POINTS_PER_CHUNK - 1) / SIMLOD_POINTS_PER_CHUNK;
+        if (npc > ROW_SLOTS) return fail(SIMLOD_ERR_CAPACITY, "%s: record %u holds %u point chunks, a leaf's chunk row holds %u", path, i, npc, ROW_SLOTS);
+        plan[i].chunk = chunks;
+        plan[i].counter = counters[i];
+        plan[i].row = npc ? ++out->numRows : 0;
+        plan[i].grid = i == 0 ? 16 : inner ? ++innerNonRoot : 0;        // grid index for now, offset below
+        chunks += npc + (r.num_voxels + SIMLOD_POINTS_PER_CHUNK - 1) / SIMLOD_POINTS_PER_CHUNK;
+    }
+    if (next != n) return bad(next < n ? next : n - 1, "records that no parent reaches");
+    if (maxLevel != h.info.max_level || samples != h.info.num_samples || points != h.info.num_points || voxels != h.info.num_voxels)
+        return fail(SIMLOD_ERR_INVALID, "%s: the records' counts disagree with the header", path);
+    if (out->numRows > ROW_CAP) return fail(SIMLOD_ERR_CAPACITY, "%s: %u leaves hold points, the builder's chunk rows hold %u", path, out->numRows, ROW_CAP);
+    out->gridBase = 16 + SIMLOD_GRID_STRIDE;
+    out->chunkBase = out->gridBase + (uint64_t)innerNonRoot * SIMLOD_GRID_STRIDE;
+    out->heapEnd = out->chunkBase + chunks * SIMLOD_CHUNK_STRIDE;
+    out->numChunks = chunks;
+    out->numGrids = innerNonRoot;
+    for (uint32_t i = 1; i < n; i++) if (plan[i].grid) plan[i].grid = out->gridBase + (plan[i].grid - 1) * SIMLOD_GRID_STRIDE;
+    plan[n].chunk = chunks;
+    s.numNodes = n;
+    s.numAllocatedChunks = s.chunkPoolSize = s.numChunksPoints;     // every point chunk in use, none free
+    s.allocatedBytes_persistent = out->heapEnd;
+    s.batchletIndex = h.batchlet_index;
+    s.numPointsProcessed = h.num_points_processed;
+    return SIMLOD_OK;
+}
+
+// chunk of the plan that holds sample `x` (x < total samples)
+uint64_t chunkOfSample(const SimlodExportNode* rec, const std::vector<ImportPlan>& plan, uint32_t n, uint64_t x) {
+    uint32_t lo = 0, hi = n;                                          // the last record whose sample_offset <= x
+    while (hi - lo > 1) { const uint32_t mid = (lo + hi) / 2; if (rec[mid].sample_offset <= x) lo = mid; else hi = mid; }
+    const uint64_t local = x - rec[lo].sample_offset;
+    const uint32_t np = rec[lo].num_points, npc = (np + SIMLOD_POINTS_PER_CHUNK - 1) / SIMLOD_POINTS_PER_CHUNK;
+    return plan[lo].chunk + (local < np ? local / SIMLOD_POINTS_PER_CHUNK : npc + (local - np) / SIMLOD_POINTS_PER_CHUNK);
+}
+
+bool preadAll(int fd, char* dst, uint64_t bytes, uint64_t at) {
+    while (bytes) {
+        const ssize_t r = pread(fd, dst, bytes, (off_t)at);
+        if (r <= 0) return false;
+        dst += r; at += (uint64_t)r; bytes -= (uint64_t)r;
+    }
+    return true;
+}
+
+int loadOctree(SimlodContext* ctx, const char* path, int loader_threads, SimlodExportInfo* info, float* kernel_ms) {
+    int rc = setCurrent(ctx); if (rc) return rc;
+    if (!path) return fail(SIMLOD_ERR_INVALID, "null path");
+    if (!ctx->programs[SIMLOD_PROGRAM_CONSTRUCT].builtin)
+        return fail(SIMLOD_ERR_MODULE, "%s: not loaded, the builder's side tables are those of the built-in construct program and another one is in use", path);
+    // ---- everything that can be refused is found before the context is written -------------------------------------
+    SimlodOctreeFileHeader h;
+    rc = readOctreeHeader(path, &h); if (rc) return rc;
+    const uint32_t n = h.info.num_nodes;
+    const uint32_t maxRecords = (uint32_t)std::min<uint64_t>(ctx->buf.nodes_bytes / sizeof(SimlodNode), NODE_TABLE_CAP);
+    if (n > maxRecords) return fail(SIMLOD_ERR_CAPACITY, "%s holds %u nodes, nodes[] holds %u", path, n, maxRecords);
+    int fd = open(path, O_RDONLY);
+    if (fd < 0) return fail(SIMLOD_ERR_INVALID, "cannot open %s", path);
+    struct FdCloser { int fd; ~FdCloser() { close(fd); } } fdCloser{fd};
+    std::vector<uint8_t> head(h.samples_offset);
+    if (!preadAll(fd, (char*)head.data(), head.size(), 0)) return fail(SIMLOD_ERR_INVALID, "read error in %s", path);
+    const SimlodExportNode* rec = (const SimlodExportNode*)(head.data() + h.records_offset);
+    const uint32_t* counters = (const uint32_t*)(head.data() + h.counters_offset);
+    LoadPlan lp;
+    rc = planLoad(path, h, rec, counters, &lp); if (rc) return rc;
+    if (lp.heapEnd + HEAP_GUARD_BYTES >= ctx->buf.persistent_bytes)
+        return fail(SIMLOD_ERR_CAPACITY, "%s needs %llu heap bytes, the persistent buffer holds %llu of which the capacity guard keeps the last %llu free", path,
+                    (unsigned long long)lp.heapEnd, (unsigned long long)ctx->buf.persistent_bytes, (unsigned long long)HEAP_GUARD_BYTES);
+    const uint64_t tableBytes = align16((uint64_t)maxRecords * sizeof(SimlodExportNode)) + align16((uint64_t)(maxRecords + 1) * sizeof(ImportPlan)) + 16;
+    if (ctx->fileTablesBytes < tableBytes) {
+        if (ctx->fileTables) CU(D(cuMemFree)(ctx->fileTables));
+        ctx->fileTables = 0;
+        ctx->fileTablesBytes = 0;
+        CU(D(cuMemAlloc)(&ctx->fileTables, tableBytes));
+        ctx->fileTablesBytes = tableBytes;
+    }
+    rc = ensureFileWindow(ctx); if (rc) return rc;
+
+    // ---- the context's octree is replaced from here on ------------------------------------------------------------------
+    CU(D(cuStreamSynchronize)(ctx->streamCopy));
+    CU(D(cuStreamSynchronize)(ctx->streamUpload));
+    CU(D(cuStreamSynchronize)(ctx->streamMain));
+    for (int i = 0; i < 3; i++) { ctx->uniforms.boxMin[i] = h.box_min[i]; ctx->uniforms.boxMax[i] = h.box_max[i]; }
+    ImportArgs a{};
+    a.nodes = ctx->buf.nodes; a.heap = ctx->buf.persistent; a.scratch = ctx->buf.momentary;
+    a.rec = ctx->fileTables;
+    a.plan = a.rec + align16((uint64_t)maxRecords * sizeof(SimlodExportNode));
+    a.error = a.plan + align16((uint64_t)(maxRecords + 1) * sizeof(ImportPlan));
+    a.chunkBase = lp.chunkBase; a.numRecords = n; a.numRows = lp.numRows;
+    for (int i = 0; i < 3; i++) { a.boxMin[i] = h.box_min[i]; a.boxMax[i] = h.box_max[i]; }
+    const SimlodHeapHeader heapHeader{(uint8_t*)(uintptr_t)ctx->buf.persistent, lp.heapEnd};
+    CU(D(cuMemsetD8Async)(ctx->buf.nodes, 0, ctx->buf.nodes_bytes, ctx->streamMain));
+    CU(D(cuMemcpyHtoDAsync)(a.rec, rec, (size_t)n * sizeof(SimlodExportNode), ctx->streamMain));
+    CU(D(cuMemcpyHtoDAsync)(a.plan, lp.plan.data(), lp.plan.size() * sizeof(ImportPlan), ctx->streamMain));
+    CU(D(cuMemsetD32Async)(a.error, 0, 1, ctx->streamMain));
+    CU(D(cuMemcpyHtoDAsync)(ctx->buf.persistent, &heapHeader, sizeof(heapHeader), ctx->streamMain));
+    CU(D(cuEventRecord)(ctx->evStart, ctx->streamMain));
+    const unsigned blocks = (unsigned)ctx->numSMs * 4;
+    { void* args[] = {&a};
+      CU(D(cuLaunchKernel)(ctx->fnImportNodes, blocks, 1, 1, 256, 1, 1, 0, ctx->streamMain, args, nullptr)); }
+    uint64_t numChunks = lp.numChunks, gridBase = lp.gridBase;
+    uint32_t numGrids = lp.numGrids;
+    CUdeviceptr heap = ctx->buf.persistent;
+    { void* args[] = {&a, &numChunks};
+      CU(D(cuLaunchKernel)(ctx->fnImportLink, blocks, 1, 1, 256, 1, 1, 0, ctx->streamMain, args, nullptr)); }
+    { void* args[] = {&heap, &gridBase, &numGrids};
+      CU(D(cuLaunchKernel)(ctx->fnImportClearGrids, blocks * 2, 1, 1, 256, 1, 1, 0, ctx->streamMain, args, nullptr)); }
+    CU(D(cuEventRecord)(ctx->evEnd, ctx->streamMain));
+    ctx->launches += 3;
+    // samples: loader threads read window w into pool half w & 1 while window w - 1 is copied and scattered
+    const uint64_t numSamples = h.info.num_samples;
+    const uint64_t numWindows = (numSamples + FILE_WINDOW_SAMPLES - 1) / FILE_WINDOW_SAMPLES;
+    SimlodContext::LaunchQueue& q = ctx->queue;
+    float ms = 0.0f, t = 0.0f;
+    const int nThreads = std::max(1, std::min(loader_threads, 64));
+    if (!ctx->loaderPool) ctx->loaderPool = new LoaderPool();
+    LoaderPool* pool = ctx->loaderPool;
+    bool readFailed = false;
+    auto retire = [&](uint64_t w) -> int {           // the scatter of window w (and the copy before it) has completed
+        CU(D(cuEventSynchronize)(q.ev[w & 1][1]));
+        float g = 0.0f;
+        CU(D(cuEventElapsedTime)(&g, q.ev[w & 1][0], q.ev[w & 1][1]));
+        ms += g;
+        return SIMLOD_OK;
+    };
+    for (uint64_t w = 0; w < numWindows && !readFailed; w++) {
+        const uint64_t first = w * FILE_WINDOW_SAMPLES, count = std::min<uint64_t>(FILE_WINDOW_SAMPLES, numSamples - first);
+        char* dst = (char*)ctx->pinnedPool + (w & 1) * FILE_WINDOW_BYTES;
+        if (w >= 2) { rc = retire(w - 2); if (rc) return rc; }
+        const uint64_t bytes = count * sizeof(SimlodPoint), at = h.samples_offset + first * sizeof(SimlodPoint);
+        const uint64_t pieces = (bytes + PIECE_BYTES - 1) / PIECE_BYTES;
+        std::atomic<uint64_t> nextPiece{0};
+        std::atomic<bool> ok{true};
+        pool->run(nThreads, [&, pool](int worker) {
+            char* stage = pool->bounce[worker];
+            for (uint64_t piece; (piece = nextPiece.fetch_add(1)) < pieces && ok.load();) {
+                const uint64_t p0 = piece * PIECE_BYTES, pn = std::min<uint64_t>(PIECE_BYTES, bytes - p0);
+                for (uint64_t done = 0; done < pn;) {
+                    const uint64_t want = std::min<uint64_t>(pn - done, LoaderPool::BOUNCE_BYTES);
+                    if (!preadAll(fd, stage, want, at + p0 + done)) { ok.store(false); break; }
+                    copyStreaming(dst + p0 + done, stage, want);          // want is a multiple of 16
+                    done += want;
+                }
+            }
+        });
+        pool->wait();
+        if (!ok.load()) { readFailed = true; break; }
+        CU(D(cuMemcpyHtoDAsync)(ctx->fileWindow, dst, (size_t)bytes, ctx->streamMain));
+        uint64_t winBegin = first, winEnd = first + count;
+        uint64_t chunk0 = chunkOfSample(rec, lp.plan, n, winBegin), chunk1 = chunkOfSample(rec, lp.plan, n, winEnd - 1) + 1;
+        CUdeviceptr window = ctx->fileWindow;
+        CU(D(cuEventRecord)(q.ev[w & 1][0], ctx->streamMain));
+        { void* args[] = {&a, &window, &winBegin, &winEnd, &chunk0, &chunk1};
+          CU(D(cuLaunchKernel)(ctx->fnImportScatter, blocks * 2, 1, 1, 256, 1, 1, 0, ctx->streamMain, args, nullptr)); }
+        CU(D(cuEventRecord)(q.ev[w & 1][1], ctx->streamMain));
+        ctx->launches++;
+    }
+    if (!readFailed) {
+        // the voxels against the grids the points rebuilt: membership, then the two flip passes, then the counts
+        CU(D(cuEventRecord)(q.ev[2][0], ctx->streamMain));
+        for (uint32_t mode = 0; mode < 3; mode++) {
+            void* args[] = {&a, &numChunks, &mode};
+            CU(D(cuLaunchKernel)(ctx->fnImportVoxels, blocks * 2, 1, 1, 256, 1, 1, 0, ctx->streamMain, args, nullptr));
+        }
+        { void* args[] = {&a};
+          CU(D(cuLaunchKernel)(ctx->fnImportCountGrids, blocks * 2, 1, 1, 256, 1, 1, 0, ctx->streamMain, args, nullptr)); }
+        CU(D(cuEventRecord)(q.ev[2][1], ctx->streamMain));
+        ctx->launches += 4;
+    }
+    CU(D(cuStreamSynchronize)(ctx->streamMain));
+    for (uint64_t w = numWindows >= 2 ? numWindows - 2 : 0; w < numWindows && !readFailed; w++) { rc = retire(w); if (rc) return rc; }
+    CU(D(cuEventElapsedTime)(&t, ctx->evStart, ctx->evEnd));
+    ms += t;
+    if (!readFailed) { CU(D(cuEventElapsedTime)(&t, q.ev[2][0], q.ev[2][1])); ms += t; }
+    uint32_t error = 0;
+    CU(D(cuMemcpyDtoH)(&error, a.error, 4));
+    if (readFailed || error) {
+        rc = simlod_reset(ctx); if (rc) return rc;                   // an empty octree in the file's box
+        if (readFailed) return fail(SIMLOD_ERR_INVALID, "read error in %s; the context holds an empty octree", path);
+        return fail(SIMLOD_ERR_INVALID, "%s: samples do not fit their nodes (error %u: 1 a point outside its leaf, 2 a voxel off the centre of its points' cells, 4 two voxels in one cell, 8 a node with other than one voxel per cell its points occupy); the context holds an empty octree", path, error);
+    }
+    // Stats, and the ring: the next batch is batch batchletIndex, in slot batchletIndex % 50
+    SimlodStats st = lp.stats;
+    st.frameID = (uint32_t)ctx->frameCounter;
+    st.allocatedBytes_momentary = scratch::TOTAL;                    // as every kernel_construct launch reports it
+    CU(D(cuMemcpyHtoD)(ctx->buf.stats, &st, sizeof(st)));
+    *ctx->hStats = st;
+    CU(D(cuMemsetD32Async)(ctx->numBatchesUploaded, h.batchlet_index, 1, ctx->streamMain));
+    CU(D(cuMemsetD8Async)(ctx->batchSizes, 0, 4 * RING_SLOTS, ctx->streamMain));
+    CU(D(cuStreamSynchronize)(ctx->streamMain));
+    ctx->uploaded = ctx->processed = h.batchlet_index;
+    ctx->unpublished = 0;
+    memset(ctx->hostSizes, 0, sizeof(ctx->hostSizes));
+    if (info) *info = h.info;
+    if (kernel_ms) *kernel_ms = ms;
+    return SIMLOD_OK;
+}
+}  // namespace
+
+extern "C" {
+
+int simlod_read_octree_header(const char* path, SimlodOctreeFileHeader* out) {
+    if (!path || !out) return fail(SIMLOD_ERR_INVALID, "null argument");
+    return readOctreeHeader(path, out);
+}
+
+int simlod_save_octree(SimlodContext* ctx, const char* path, SimlodExportInfo* info, float* kernel_ms) {
+    return saveOctree(ctx, path, info, kernel_ms);
+}
+
+int simlod_load_octree(SimlodContext* ctx, const char* path, int loader_threads, SimlodExportInfo* info, float* kernel_ms) {
+    return loadOctree(ctx, path, loader_threads, info, kernel_ms);
 }
 
 // ---- spatial exchange (SURVEY.md §8f-3); kernels in partition.cu ----------------------------------------
