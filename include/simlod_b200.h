@@ -196,6 +196,54 @@ int simlod_export_octree(SimlodContext* ctx, int32_t depth, uint64_t dst_nodes, 
 int simlod_export_view(SimlodContext* ctx, uint64_t dst_nodes, uint64_t node_capacity, uint64_t dst_samples,
                        uint64_t sample_capacity, SimlodExportInfo* info, float* kernel_ms);
 
+// Region query (DESIGN.md §9.8): the samples of the octree inside a box, a sphere or a convex set of half-spaces, filtered
+// on the device into a flat array of 16-byte SimlodPoint samples. Coordinates are those of the stored samples (the ones
+// the insert calls received, the box of simlod_set_uniforms).
+enum { SIMLOD_REGION_BOX = 1, SIMLOD_REGION_SPHERE = 2, SIMLOD_REGION_PLANES = 3 };
+#define SIMLOD_REGION_MAX_PLANES 16
+typedef struct SimlodRegion {
+    uint32_t kind, num_planes;                      //   0  SIMLOD_REGION_*; planes in use (PLANES only)
+    float    box_min[3], box_max[3];                //   8  BOX:    min <= p <= max on every axis
+    float    center[3], radius;                     //  32  SPHERE: |p - center|^2 <= radius^2
+    float    planes[SIMLOD_REGION_MAX_PLANES][4];   //  48  PLANES: n.p + d >= 0 for each of the first num_planes, (nx, ny, nz, d)
+} SimlodRegion;
+typedef struct SimlodQueryInfo {
+    uint64_t num_samples, num_points, num_voxels;   //   0  returned
+    uint64_t samples_tested;                        //  24  samples of the visited nodes, each put through the per-sample test
+    uint32_t nodes_visited;                         //  32  sampled nodes the region may touch (the rest were skipped unread)
+    uint32_t max_level;                             //  36  deepest level in the octree
+} SimlodQueryInfo;
+SIMLOD_STATIC_ASSERT(sizeof(SimlodRegion) == 304, "Region");
+SIMLOD_STATIC_ASSERT(offsetof(SimlodRegion, box_min) == 8 && offsetof(SimlodRegion, box_max) == 20, "Region.box");
+SIMLOD_STATIC_ASSERT(offsetof(SimlodRegion, center) == 32 && offsetof(SimlodRegion, radius) == 44, "Region.sphere");
+SIMLOD_STATIC_ASSERT(offsetof(SimlodRegion, planes) == 48, "Region.planes");
+SIMLOD_STATIC_ASSERT(sizeof(SimlodQueryInfo) == 40, "QueryInfo");
+SIMLOD_STATIC_ASSERT(offsetof(SimlodQueryInfo, samples_tested) == 24 && offsetof(SimlodQueryInfo, nodes_visited) == 32, "QueryInfo.samples_tested");
+//   sample set   depth < 0: the points of every leaf, i.e. the inserted point set, no voxels. 0 <= depth <= 20: the cut of
+//                simlod_export_octree at `depth` (the voxels of each inner node at level == depth, the points of each
+//                leaf at level <= depth), so a coarse preview of a region costs a coarse amount of work
+//   result       exactly those samples of the set that pass the region's predicate above and are eligible (below),
+//                bit for bit as stored. Order: nodes in the export's breadth-first (level, Morton) order, within a node in
+//                chunk-list order; two queries of the same buffers are byte-identical
+//   predicates   evaluated in float32 without contraction: six comparisons for the box;
+//                (x-cx)*(x-cx) + (y-cy)*(y-cy) + (z-cz)*(z-cz) <= r*r, summed left to right, for the sphere;
+//                ((nx*x + ny*y) + nz*z) + d >= 0 for each plane, used as given (not normalised)
+//   eligible     a point is eligible when on every axis it is not below boxMin and its lattice coordinate, the builder's
+//                u32(2^20 * (p - boxMin) * rcp(cubeSize)), is below 2^20. The builder files a point outside that
+//                half-open cube under a wrapped or saturated coordinate, so no node's box bounds it and no hierarchical
+//                skip could be exact for it: such points (in practice those exactly on the max face of the longest axis)
+//                are never returned. Voxel centres are always eligible.
+// A node whose box, inflated by a rounding margin, cannot hold an eligible sample that passes is skipped with its
+// subtree, unread; every sample of the other (visited) nodes is tested. dst_samples == 0 fills *info only (size query).
+// SIMLOD_ERR_INVALID, before any launch, for depth > 20, a misaligned destination or a malformed region (unknown kind,
+// num_planes 0 or > 16, a non-finite number, box_min > box_max on an axis, a negative radius); with nothing written,
+// for a capacity below info->num_samples or an inconsistent image in the part of the octree the query visits (the
+// export's conditions). Reads the ABI only, as the export does, and writes nothing into the context's buffers or Stats.
+// Enqueued on the launch stream; returns once complete. *kernel_ms (optional) = event time of the query kernels. Scratch
+// memory is the context's (shared with the exports), kept until simlod_destroy.
+int simlod_query_region(SimlodContext* ctx, const SimlodRegion* region, int32_t depth, uint64_t dst_samples,
+                        uint64_t sample_capacity, SimlodQueryInfo* info, float* kernel_ms);
+
 // Octree files (SimlodOctreeFileHeader, DESIGN.md §9.7): a built octree saved and loaded back, so that it can be rendered,
 // exported or continued with new batches in another context, process or session.
 // simlod_read_octree_header: the header of an octree file, checked against itself and the file size. No context, no GPU.

@@ -134,6 +134,53 @@ class OctreeFileHeader(C.Structure):
                 ("samples_offset", C.c_uint64), ("file_size", C.c_uint64), ("reserved1", C.c_uint64)]
 
 
+REGION_BOX, REGION_SPHERE, REGION_PLANES = 1, 2, 3
+REGION_MAX_PLANES = 16
+
+
+class SimlodRegion(C.Structure):
+    """SimlodRegion: a box, a sphere or up to 16 half-spaces, in the coordinates of the stored samples."""
+    _fields_ = [("kind", C.c_uint32), ("num_planes", C.c_uint32), ("box_min", C.c_float * 3), ("box_max", C.c_float * 3),
+                ("center", C.c_float * 3), ("radius", C.c_float), ("planes", (C.c_float * 4) * REGION_MAX_PLANES)]
+
+
+class SimlodQueryInfo(C.Structure):
+    """SimlodQueryInfo: what a region query returned and how much of the octree it had to look at."""
+    _fields_ = [("num_samples", C.c_uint64), ("num_points", C.c_uint64), ("num_voxels", C.c_uint64), ("samples_tested", C.c_uint64),
+                ("nodes_visited", C.c_uint32), ("max_level", C.c_uint32)]
+
+
+class Region:
+    """Constructors of the regions SimLOD.query_region takes. Numbers are rounded to float32, the type the predicates are
+    evaluated in; a malformed region (non-finite number, min > max, negative radius) is refused by the query."""
+
+    @staticmethod
+    def box(mn, mx):
+        """min <= p <= max on every axis."""
+        r = SimlodRegion(kind=REGION_BOX)
+        r.box_min[:] = [float(v) for v in mn]
+        r.box_max[:] = [float(v) for v in mx]
+        return r
+
+    @staticmethod
+    def sphere(center, radius):
+        """|p - center|^2 <= radius^2."""
+        r = SimlodRegion(kind=REGION_SPHERE, radius=float(radius))
+        r.center[:] = [float(v) for v in center]
+        return r
+
+    @staticmethod
+    def planes(planes):
+        """n.p + d >= 0 for every row (nx, ny, nz, d) of a (k, 4) array, 1 <= k <= 16; rows are used as given."""
+        a = np.asarray(planes, dtype=np.float32)
+        if a.ndim != 2 or a.shape[1] != 4 or not 1 <= a.shape[0] <= REGION_MAX_PLANES:
+            raise ValueError("planes must be a (k, 4) array with 1 <= k <= %d" % REGION_MAX_PLANES)
+        r = SimlodRegion(kind=REGION_PLANES, num_planes=a.shape[0])
+        for k in range(a.shape[0]):
+            r.planes[k][:] = [float(v) for v in a[k]]
+        return r
+
+
 class OctreeExport:
     """SimLOD.export_octree() / export_view(): `nodes` (EXPORT_NODE_DTYPE records, breadth-first), `samples` (the sample
     array), `info`."""
@@ -146,6 +193,7 @@ assert C.sizeof(Uniforms) == 480 and C.sizeof(Stats) == 112
 assert C.sizeof(ExportInfo) == 32 and EXPORT_NODE_DTYPE.itemsize == 64
 assert C.sizeof(LasHeader) == 128
 assert C.sizeof(OctreeFileHeader) == 128
+assert C.sizeof(SimlodRegion) == 304 and C.sizeof(SimlodQueryInfo) == 40
 
 # every symbol include/simlod_b200.h declares
 EXPORTS = [
@@ -158,7 +206,7 @@ EXPORTS = [
     "simlod_partition_count", "simlod_partition_scatter", "simlod_partition_wait",
     "simlod_export_framebuffer", "simlod_peer_signal", "simlod_composite_framebuffers", "simlod_generate", "simlod_reset_with_grid", "simlod_insert_simlod_file_ex", "simlod_get_numa_node",
     "simlod_export_octree", "simlod_export_view", "simlod_read_las_header", "simlod_insert_files",
-    "simlod_read_octree_header", "simlod_save_octree", "simlod_load_octree",
+    "simlod_read_octree_header", "simlod_save_octree", "simlod_load_octree", "simlod_query_region",
 ]
 
 _lib = None
@@ -221,6 +269,7 @@ def load_library():
         "simlod_read_octree_header": [C.c_char_p, C.POINTER(OctreeFileHeader)],
         "simlod_save_octree": [vp, C.c_char_p, C.POINTER(ExportInfo), C.POINTER(C.c_float)],
         "simlod_load_octree": [vp, C.c_char_p, C.c_int, C.POINTER(ExportInfo), C.POINTER(C.c_float)],
+        "simlod_query_region": [vp, C.POINTER(SimlodRegion), C.c_int32, u64, u64, C.POINTER(SimlodQueryInfo), C.POINTER(C.c_float)],
     }
     for name, argtypes in sig.items():
         fn = getattr(lib, name)
@@ -579,6 +628,45 @@ class SimLOD:
         info, _ = into(nodes_t.data_ptr(), n, samples.data_ptr() if m else 0, m)
         nodes = nodes_t.cpu().numpy().view(EXPORT_NODE_DTYPE)
         return OctreeExport(nodes, samples, info)
+
+    def query_region_into(self, region, depth, dst_samples, sample_capacity):
+        """simlod_query_region into caller-owned device memory (depth None or < 0: the inserted points; dst_samples 0:
+        size query). Returns (SimlodQueryInfo, kernel ms)."""
+        info, ms = SimlodQueryInfo(), C.c_float(0)
+        d = -1 if depth is None else int(depth)
+        self._check(self._lib.simlod_query_region(self._ctx, C.byref(region), d, int(dst_samples), int(sample_capacity),
+                                                  C.byref(info), C.byref(ms)))
+        return info, ms.value
+
+    def query_region(self, region, depth=None, device="cuda"):
+        """The samples inside `region` (Region.box / sphere / planes), filtered on the GPU (simlod_query_region): with
+        depth=None the inserted points, with an integer depth the samples of the cut at that level (as export_octree), so
+        that a coarse preview costs a coarse amount of work. Points outside the half-open octree cube (in practice those
+        exactly on its max face) are never returned. The order is deterministic. Returns (samples, SimlodQueryInfo):
+        with device="cuda" a float32 torch tensor of shape (N, 4) in device memory (x, y, z, colour bits), with
+        device="cpu" a numpy POINT_DTYPE array."""
+        info, _ = self.query_region_into(region, depth, 0, 0)
+        m = info.num_samples
+        if device == "cpu":
+            ds = self.device_alloc(m * 16) if m else 0
+            try:
+                if m:
+                    info, _ = self.query_region_into(region, depth, ds, m)
+                return self.memcpy_dtoh(ds, m * 16).view(POINT_DTYPE), info
+            finally:
+                if ds:
+                    self.device_free(ds)
+        import torch
+        dev = torch.device(device)
+        if dev.type != "cuda":
+            raise ValueError("device must be 'cpu' or a CUDA device, not %r" % device)
+        if dev.index is None:
+            dev = torch.device("cuda", self.device)
+        samples = torch.empty((m, 4), dtype=torch.float32, device=dev)
+        torch.cuda.current_stream(dev).synchronize()       # the caching allocator may hand out memory torch still uses
+        if m:
+            info, _ = self.query_region_into(region, depth, samples.data_ptr(), m)
+        return samples, info
 
     def host_alloc(self, nbytes):
         p = C.c_void_p()

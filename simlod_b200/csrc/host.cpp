@@ -33,6 +33,7 @@
 #include <cctype>
 #include <cstring>
 #include <fstream>
+#include <cmath>
 #include <string>
 #include <vector>
 
@@ -46,6 +47,7 @@ extern const unsigned char simlod_cubin_las[];
 extern const unsigned char simlod_cubin_gen[];
 extern const unsigned char simlod_cubin_export[];
 extern const unsigned char simlod_cubin_import[];
+extern const unsigned char simlod_cubin_query[];
 }
 
 namespace {
@@ -169,8 +171,10 @@ struct SimlodContext {
                fnExportPlanView = nullptr;
     CUdeviceptr exportScratch = 0;     // octree export: records | node indices | first items | chunk items | ExportCtl
     uint64_t exportScratchBytes = 0;
-    void* hExportCtl = nullptr;        // pinned copy of ExportCtl
+    void* hExportCtl = nullptr;        // pinned copy of ExportCtl / QueryCtl (CTL_HOST_BYTES)
     CUfunction fnExportGatherWindow = nullptr, fnExportCounters = nullptr;
+    CUmodule queryModule = nullptr;    // region query (query.cu); shares exportScratch, hExportCtl and fnExportCollect
+    CUfunction fnQueryPlan = nullptr, fnQueryCount = nullptr, fnQueryScan = nullptr, fnQueryWrite = nullptr;
     CUmodule importModule = nullptr;
     CUfunction fnImportNodes = nullptr, fnImportLink = nullptr, fnImportClearGrids = nullptr, fnImportScatter = nullptr,
                fnImportVoxels = nullptr, fnImportCountGrids = nullptr;
@@ -470,6 +474,11 @@ static int createResources(SimlodContext* ctx, const SimlodConfig* config) {
     CU(D(cuModuleGetFunction)(&ctx->fnExportPlanView, ctx->exportModule, "simlod_export_plan_view"));
     CU(D(cuModuleGetFunction)(&ctx->fnExportGatherWindow, ctx->exportModule, "simlod_export_gather_window"));
     CU(D(cuModuleGetFunction)(&ctx->fnExportCounters, ctx->exportModule, "simlod_export_counters"));
+    CU(D(cuModuleLoadData)(&ctx->queryModule, simlod_cubin_query));
+    CU(D(cuModuleGetFunction)(&ctx->fnQueryPlan, ctx->queryModule, "simlod_query_plan"));
+    CU(D(cuModuleGetFunction)(&ctx->fnQueryCount, ctx->queryModule, "simlod_query_count"));
+    CU(D(cuModuleGetFunction)(&ctx->fnQueryScan, ctx->queryModule, "simlod_query_scan"));
+    CU(D(cuModuleGetFunction)(&ctx->fnQueryWrite, ctx->queryModule, "simlod_query_write"));
     CU(D(cuModuleLoadData)(&ctx->importModule, simlod_cubin_import));
     CU(D(cuModuleGetFunction)(&ctx->fnImportNodes, ctx->importModule, "simlod_import_nodes"));
     CU(D(cuModuleGetFunction)(&ctx->fnImportLink, ctx->importModule, "simlod_import_link"));
@@ -585,6 +594,7 @@ void simlod_destroy(SimlodContext* ctx) {
             if (ctx->evStagingFree[i]) D(cuEventDestroy)(ctx->evStagingFree[i]);
         }
         if (ctx->exportModule) D(cuModuleUnload)(ctx->exportModule);
+        if (ctx->queryModule) D(cuModuleUnload)(ctx->queryModule);
         if (ctx->exportScratch) D(cuMemFree)(ctx->exportScratch);
         if (ctx->hExportCtl) D(cuMemFreeHost)(ctx->hExportCtl);
         if (ctx->importModule) D(cuModuleUnload)(ctx->importModule);
@@ -1414,6 +1424,20 @@ struct ExportViewScratch {           // mirrors export.cu ViewScratch
 };
 constexpr uint64_t align16(uint64_t v) { return (v + 15) & ~15ull; }
 
+// The context's export / query scratch, grown to `bytes`, and the pinned copy of the control word.
+constexpr size_t CTL_HOST_BYTES = 128;
+int exportScratch(SimlodContext* ctx, uint64_t bytes) {
+    if (ctx->exportScratchBytes < bytes) {
+        if (ctx->exportScratch) CU(D(cuMemFree)(ctx->exportScratch));
+        ctx->exportScratch = 0;
+        ctx->exportScratchBytes = 0;
+        CU(D(cuMemAlloc)(&ctx->exportScratch, bytes));
+        ctx->exportScratchBytes = bytes;
+    }
+    if (!ctx->hExportCtl) CU(D(cuMemHostAlloc)(&ctx->hExportCtl, CTL_HOST_BYTES, 0));
+    return SIMLOD_OK;
+}
+
 // Stage 1 of an export, into scratch only: the view's drawn flags, the plan and the chunk-list walk. On success p holds
 // the checked ExportCtl and where the records, node indices, chunk items and ExportCtl lie.
 struct ExportPlanned {
@@ -1432,14 +1456,7 @@ int exportPlan(SimlodContext* ctx, int32_t depth, const SimlodUniforms* view, Ex
                    offIndex = offMark + align16(maxRecords), offViewRec = offIndex + align16((uint64_t)maxRecords * 4),
                    offViewNode = offViewRec + align16((uint64_t)maxRecords * sizeof(SimlodExportNode)),
                    bytes = view ? offViewNode + align16((uint64_t)maxRecords * 4) : offCtl + sizeof(ExportCtl);
-    if (ctx->exportScratchBytes < bytes) {
-        if (ctx->exportScratch) CU(D(cuMemFree)(ctx->exportScratch));
-        ctx->exportScratch = 0;
-        ctx->exportScratchBytes = 0;
-        CU(D(cuMemAlloc)(&ctx->exportScratch, bytes));
-        ctx->exportScratchBytes = bytes;
-    }
-    if (!ctx->hExportCtl) CU(D(cuMemHostAlloc)(&ctx->hExportCtl, sizeof(ExportCtl), 0));
+    int rc = exportScratch(ctx, bytes); if (rc) return rc;
     CUdeviceptr nodes = ctx->buf.nodes, heap = ctx->buf.persistent, stats = ctx->buf.stats;
     CUdeviceptr rec = ctx->exportScratch, recNode = rec + offNode, recItem = rec + offItem, items = rec + offItems, ctl = rec + offCtl;
     ExportViewScratch vs{};
@@ -1522,6 +1539,100 @@ int simlod_export_view(SimlodContext* ctx, uint64_t dst_nodes, uint64_t node_cap
                        uint64_t sample_capacity, SimlodExportInfo* info, float* kernel_ms) {
     if (!ctx) return fail(SIMLOD_ERR_INVALID, "null context");
     return exportOctree(ctx, -1, &ctx->uniforms, dst_nodes, node_capacity, dst_samples, sample_capacity, info, kernel_ms);
+}
+
+// ---- region query (DESIGN.md §9.8); kernels in query.cu, the chunk-list walk is export.cu's ----------------------------
+namespace {
+struct QueryCtl {                    // mirrors query.cu
+    ExportCtl plan;
+    uint64_t outSamples, outPoints, outVoxels;
+    uint32_t nodesVisited, pad;
+};
+static_assert(sizeof(QueryCtl) <= CTL_HOST_BYTES, "pinned control word");
+struct QueryBox { float mn[3], mx[3]; };
+
+int checkRegion(const SimlodRegion* r) {
+    if (!r) return fail(SIMLOD_ERR_INVALID, "null region");
+    auto finite = [](const float* v, int n) { for (int i = 0; i < n; i++) if (!std::isfinite(v[i])) return false; return true; };
+    switch (r->kind) {
+    case SIMLOD_REGION_BOX:
+        if (!finite(r->box_min, 3) || !finite(r->box_max, 3)) return fail(SIMLOD_ERR_INVALID, "region box has a non-finite bound");
+        for (int a = 0; a < 3; a++)
+            if (r->box_min[a] > r->box_max[a]) return fail(SIMLOD_ERR_INVALID, "region box has min > max on axis %d", a);
+        return SIMLOD_OK;
+    case SIMLOD_REGION_SPHERE:
+        if (!finite(r->center, 3) || !std::isfinite(r->radius)) return fail(SIMLOD_ERR_INVALID, "region sphere has a non-finite centre or radius");
+        if (r->radius < 0.0f) return fail(SIMLOD_ERR_INVALID, "region sphere has a negative radius");
+        return SIMLOD_OK;
+    case SIMLOD_REGION_PLANES:
+        if (r->num_planes == 0 || r->num_planes > SIMLOD_REGION_MAX_PLANES)
+            return fail(SIMLOD_ERR_INVALID, "region has %u planes, 1 to %d are supported", r->num_planes, (int)SIMLOD_REGION_MAX_PLANES);
+        if (!finite(&r->planes[0][0], 4 * (int)r->num_planes)) return fail(SIMLOD_ERR_INVALID, "region has a non-finite plane coefficient");
+        return SIMLOD_OK;
+    }
+    return fail(SIMLOD_ERR_INVALID, "unknown region kind %u", r->kind);
+}
+}  // namespace
+
+int simlod_query_region(SimlodContext* ctx, const SimlodRegion* region, int32_t depth, uint64_t dst_samples,
+                        uint64_t sample_capacity, SimlodQueryInfo* info, float* kernel_ms) {
+    int rc = setCurrent(ctx); if (rc) return rc;
+    if (!info) return fail(SIMLOD_ERR_INVALID, "null info");
+    if (depth > SIMLOD_MAX_DEPTH) return fail(SIMLOD_ERR_INVALID, "query depth %d exceeds the octree's maximum depth %d", depth, (int)SIMLOD_MAX_DEPTH);
+    if (dst_samples % 16) return fail(SIMLOD_ERR_INVALID, "query destination must be 16-byte aligned");
+    rc = checkRegion(region); if (rc) return rc;
+    // the export's scratch (one record per node of nodes[], one item per chunk the heap can hold) plus one word per item
+    const uint32_t maxRecords = (uint32_t)(ctx->buf.nodes_bytes / sizeof(SimlodNode));
+    const uint64_t itemsCap = ctx->buf.persistent_bytes / SIMLOD_CHUNK_STRIDE + 1;
+    const uint64_t offNode = align16((uint64_t)maxRecords * sizeof(SimlodExportNode)), offItem = offNode + align16((uint64_t)maxRecords * 4),
+                   offItems = offItem + align16((uint64_t)maxRecords * 8), offWords = offItems + itemsCap * 16,
+                   offCtl = offWords + align16(itemsCap * 8);
+    rc = exportScratch(ctx, offCtl + sizeof(QueryCtl)); if (rc) return rc;
+    CUdeviceptr nodes = ctx->buf.nodes, heap = ctx->buf.persistent, stats = ctx->buf.stats;
+    CUdeviceptr rec = ctx->exportScratch, recNode = rec + offNode, recItem = rec + offItem, items = rec + offItems, words = rec + offWords,
+                ctl = rec + offCtl;
+    uint64_t heapBytes = ctx->buf.persistent_bytes, cap = itemsCap;
+    SimlodRegion rg = *region;
+    QueryBox box;
+    for (int a = 0; a < 3; a++) { box.mn[a] = ctx->uniforms.boxMin[a]; box.mx[a] = ctx->uniforms.boxMax[a]; }
+    // stage 1, into scratch only: plan (one block), the chunk-list walk, the per-item counts and their scan
+    CU(D(cuEventRecord)(ctx->evStart, ctx->streamMain));
+    { void* args[] = {&nodes, &stats, &depth, (void*)&maxRecords, &rec, &recNode, &recItem, &ctl, &rg, &box};
+      CU(D(cuLaunchKernel)(ctx->fnQueryPlan, 1, 1, 1, 1024, 1, 1, 0, ctx->streamMain, args, nullptr)); }
+    { void* args[] = {&nodes, &heap, &heapBytes, &rec, &recNode, &recItem, &items, &cap, &ctl};
+      CU(D(cuLaunchKernel)(ctx->fnExportCollect, (unsigned)ctx->numSMs * 2, 1, 1, 256, 1, 1, 0, ctx->streamMain, args, nullptr)); }
+    { void* args[] = {&items, &rec, &recItem, &words, &ctl, &rg, &box};
+      CU(D(cuLaunchKernel)(ctx->fnQueryCount, (unsigned)ctx->numSMs * 8, 1, 1, 256, 1, 1, 0, ctx->streamMain, args, nullptr)); }
+    { void* args[] = {&words, &ctl};
+      CU(D(cuLaunchKernel)(ctx->fnQueryScan, 1, 1, 1, 1024, 1, 1, 0, ctx->streamMain, args, nullptr)); }
+    CU(D(cuEventRecord)(ctx->evEnd, ctx->streamMain));
+    ctx->launches += 4;
+    CU(D(cuMemcpyDtoHAsync)(ctx->hExportCtl, ctl, sizeof(QueryCtl), ctx->streamMain));
+    CU(D(cuStreamSynchronize)(ctx->streamMain));
+    const QueryCtl c = *(const QueryCtl*)ctx->hExportCtl;
+    float ms = 0.0f;
+    CU(D(cuEventElapsedTime)(&ms, ctx->evStart, ctx->evEnd));
+    if (kernel_ms) *kernel_ms = ms;
+    if (c.plan.error)
+        return fail(SIMLOD_ERR_INVALID, "octree image is inconsistent (error %u: 1 child pointer outside nodes[], 2 chunk pointer outside the used heap, 4 list shorter than its count, 5 inner node without 8 children)", c.plan.error);
+    info->num_samples = c.outSamples; info->num_points = c.outPoints; info->num_voxels = c.outVoxels;
+    info->samples_tested = c.plan.numSamples; info->nodes_visited = c.nodesVisited; info->max_level = c.plan.maxLevel;
+    if (!dst_samples) return SIMLOD_OK;                         // size query
+    if (sample_capacity < c.outSamples)
+        return fail(SIMLOD_ERR_INVALID, "sample destination holds %llu samples, the query returns %llu", (unsigned long long)sample_capacity, (unsigned long long)c.outSamples);
+    if (!c.outSamples) return SIMLOD_OK;
+    // stage 2: the passing samples into the destination
+    CUdeviceptr ds = (CUdeviceptr)dst_samples;
+    CU(D(cuEventRecord)(ctx->evTotalStart, ctx->streamMain));
+    { void* args[] = {&items, &words, &ds, &ctl, &rg, &box};
+      CU(D(cuLaunchKernel)(ctx->fnQueryWrite, (unsigned)ctx->numSMs * 8, 1, 1, 256, 1, 1, 0, ctx->streamMain, args, nullptr)); }
+    CU(D(cuEventRecord)(ctx->evTotalEnd, ctx->streamMain));
+    ctx->launches++;
+    CU(D(cuEventSynchronize)(ctx->evTotalEnd));
+    float writeMs = 0.0f;
+    CU(D(cuEventElapsedTime)(&writeMs, ctx->evTotalStart, ctx->evTotalEnd));
+    if (kernel_ms) *kernel_ms = ms + writeMs;
+    return SIMLOD_OK;
 }
 
 // ---- octree files (DESIGN.md §9.7); kernels in export.cu (save) and import.cu (load) ---------------------------------
