@@ -65,7 +65,8 @@ def _stamp_matches(stamp, digest, artefacts):
 def build_native(force=False, verbose=False):
     headers = [os.path.join(ROOT, "include", "simlod_abi.h"), os.path.join(ROOT, "include", "simlod_b200.h"),
                os.path.join(CSRC, "fpmath.cuh"), os.path.join(CSRC, "lodcut.cuh"), os.path.join(CSRC, "loader_pool.h"),
-               os.path.join(CSRC, "construct_layout.cuh"), os.path.join(CSRC, "export_common.cuh"), os.path.join(CSRC, "region.cuh")]
+               os.path.join(CSRC, "construct_layout.cuh"), os.path.join(CSRC, "export_common.cuh"), os.path.join(CSRC, "region.cuh"),
+               os.path.join(CSRC, "kernel_args.h"), os.path.join(CSRC, "render_layout.cuh")]
     sources = [os.path.join(CSRC, name + ".cu") for name in PROGRAMS] + [os.path.join(CSRC, "host.cpp")]
     digest = _digest(sources + headers, " ".join(ARCH) + " -O3 -lineinfo " + repr(sorted(EXTRA_FLAGS.items())))
     stamp = os.path.join(CUBIN_DIR, "BUILD_STAMP")

@@ -1617,7 +1617,7 @@ kernel_construct(const Uniforms uniforms, Point* points, uint32_t* buffer, uint8
         // pendingBound come from the last barrier, memUsed was written before it and is not written again until every
         // block has passed this guard, and heapExact is written between two barriers while no block allocates.
         uint64_t memUsed = sh_snap.memUsed;
-        if (sh_loop.havePending && memUsed + (uint64_t)sh_snap.numSpillTotal * SIMLOD_GRID_STRIDE + sh_loop.pendingBound + 200000000ull >= uniforms.persistentBufferCapacity) {
+        if (sh_loop.havePending && memUsed + (uint64_t)sh_snap.numSpillTotal * SIMLOD_GRID_STRIDE + sh_loop.pendingBound + HEAP_GUARD_BYTES >= uniforms.persistentBufferCapacity) {
             allocateChunks();
             gridSync();
             if (first_in_grid()) ctl->heapExact = ldv(&c.heap()->offset);
@@ -1625,7 +1625,7 @@ kernel_construct(const Uniforms uniforms, Point* points, uint32_t* buffer, uint8
             gridSync();
             memUsed = ldv(&ctl->heapExact);
         }
-        const bool memCapacityReached = memUsed + 200000000ull >= uniforms.persistentBufferCapacity;
+        const bool memCapacityReached = memUsed + HEAP_GUARD_BYTES >= uniforms.persistentBufferCapacity;
         if (first_in_grid()) stats->memCapacityReached = memCapacityReached ? 1 : 0;
         if (memCapacityReached) break;
 

@@ -6,6 +6,10 @@
 #include <stdint.h>
 #include "../../include/simlod_abi.h"
 
+// The capacity guard (voxels.cu:896-912): kernel_construct stops consuming batches once the heap offset plus this many
+// bytes reaches the persistent buffer's capacity, and a loaded octree must leave them free as well.
+constexpr uint64_t HEAP_GUARD_BYTES = 200000000ull;
+
 // ------------------------------------------------------------------------------------------
 // scratch layout inside the momentary buffer (all offsets 256-byte aligned). Everything that the
 // insertion of batch b-1 reads while batch b is being counted exists twice (index = batch parity).

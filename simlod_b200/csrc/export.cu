@@ -29,16 +29,6 @@
 #include "lodcut.cuh"
 #include "export_common.cuh"
 
-// The view export's scratch (all null for the full and depth exports). The breadth-first pass writes the record of every
-// reachable node into rec / recNode here; the records the view keeps are then compacted into the plan's rec / recNode.
-struct ViewScratch {
-    const uint8_t* drawn;         // [node index] 1 when kernel_render draws the node (simlod_export_view_flags)
-    SimlodExportNode* rec;        // [record] breadth-first records of every reachable node
-    uint32_t* recNode;            // [record] their node indices
-    uint8_t* mark;                // [record] 1 when a drawn record lies strictly below
-    uint32_t* index;              // [record] position among the kept records
-};
-
 // One thread per node of nodes[]: drawn[n] = whether kernel_render draws node n for the uniforms `u`, by the renderer's own
 // test (lodcut.cuh). The uniforms come by value, as kernel_render receives them. Writes nothing into nodes[].
 extern "C" __global__ void __launch_bounds__(256)

@@ -1,25 +1,12 @@
-// export_common.cuh — what the export (export.cu) and the region query (query.cu) share: the control word, the chunk
-// item, the inconsistency codes and the block-wide scan of their one-block plan kernels.
+// export_common.cuh — what the export (export.cu) and the region query (query.cu) share: the chunk item and the
+// block-wide scan of their one-block plan kernels. The control word and its inconsistency codes are in kernel_args.h.
 #pragma once
 #include <stdint.h>
 #include "../../include/simlod_abi.h"
+#include "kernel_args.h"
 
 constexpr uint32_t PLAN_THREADS = 1024;
 constexpr uint32_t PPC = SIMLOD_POINTS_PER_CHUNK;
-
-enum : uint32_t {                         // ExportCtl::error (the canonicaliser's codes, oracle.cpp canonFromImage)
-    EXPORT_ERR_CHILD = 1,                 // a child pointer outside nodes[] (or more records than nodes: a node reached twice)
-    EXPORT_ERR_CHUNK = 2,                 // a chunk pointer outside the used heap
-    EXPORT_ERR_SHORT = 4,                 // a list shorter than its count
-    EXPORT_ERR_PARTIAL = 5,               // an inner node without all 8 children
-};
-
-struct ExportCtl {                        // mirrors host.cpp
-    uint32_t numNodes, maxLevel;
-    uint64_t numSamples, numPoints, numVoxels;
-    uint64_t numItems;
-    uint32_t error, pad;
-};
 
 struct Item { uint64_t src; uint64_t dst; };   // dst: sample index | count << 48
 

@@ -27,34 +27,9 @@
 #include "../../include/simlod_abi.h"
 #include "fpmath.cuh"
 #include "construct_layout.cuh"
+#include "kernel_args.h"
 
 constexpr uint32_t PPC = SIMLOD_POINTS_PER_CHUNK;
-
-enum : uint32_t {                         // the error word (mirrors host.cpp)
-    IMPORT_ERR_POINT = 1,                 // a point whose descent does not end in its leaf
-    IMPORT_ERR_VOXEL = 2,                 // a voxel that is not the centre of a cell of its node
-    IMPORT_ERR_DUPLICATE = 4,             // two voxels in one cell of a node
-    IMPORT_ERR_COUNT = 8,                 // a node's voxels are not as many as the cells its points occupy
-};
-
-struct ImportPlan {                       // per record, mirrors host.cpp; one more entry after the last record (chunk = total)
-    uint64_t grid;                        // heap offset of the node's grid (0: none)
-    uint64_t chunk;                       // index of its first chunk: points first, then voxels
-    uint32_t row;                         // its chunk row (+1; 0: none)
-    uint32_t counter;                     // Node::counter from the file
-};
-
-struct ImportArgs {                       // mirrors host.cpp
-    SimlodNode* nodes;
-    uint8_t* heap;
-    uint8_t* scratch;                     // kernel_construct's momentary buffer
-    const SimlodExportNode* rec;
-    const ImportPlan* plan;
-    uint32_t* error;
-    uint64_t chunkBase;                   // heap offset of chunk 0
-    uint32_t numRecords, numRows;
-    float boxMin[3], boxMax[3];
-};
 
 __device__ __forceinline__ uint32_t ceilChunks(uint32_t n) { return (n + PPC - 1) / PPC; }
 template <typename T> __device__ __forceinline__ T* table(const ImportArgs& a, uint64_t off) { return reinterpret_cast<T*>(a.scratch + off); }

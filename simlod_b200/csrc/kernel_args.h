@@ -1,0 +1,114 @@
+// kernel_args.h — the argument and control structs that host.cpp fills and the kernels read, with the codes and limits
+// both sides use. One definition for both compilers: plain C++ (no device code), included by host.cpp and by export.cu,
+// query.cu (through export_common.cuh), import.cu and partition.cu. The static_asserts pin every size, and the offsets
+// that one side reads of a struct the other writes, so a layout change fails to compile instead of shifting bytes.
+#pragma once
+#include <stddef.h>
+#include <stdint.h>
+#include "../../include/simlod_abi.h"
+
+// ---- octree export (export.cu) and region query (query.cu) ---------------------------------------------------------
+
+enum : uint32_t {                         // ExportCtl::error (the canonicaliser's codes, oracle.cpp canonFromImage)
+    EXPORT_ERR_CHILD = 1,                 // a child pointer outside nodes[] (or more records than nodes: a node reached twice)
+    EXPORT_ERR_CHUNK = 2,                 // a chunk pointer outside the used heap
+    EXPORT_ERR_SHORT = 4,                 // a list shorter than its count
+    EXPORT_ERR_PARTIAL = 5,               // an inner node without all 8 children
+};
+
+struct ExportCtl {                        // the plan's sizes and error, read back by the host before the gather
+    uint32_t numNodes, maxLevel;
+    uint64_t numSamples, numPoints, numVoxels;
+    uint64_t numItems;
+    uint32_t error, pad;
+};
+static_assert(sizeof(ExportCtl) == 48 && offsetof(ExportCtl, numItems) == 32 && offsetof(ExportCtl, error) == 40, "ExportCtl");
+
+// The view export's scratch (all null for the full and depth exports). The breadth-first pass writes the record of every
+// reachable node into rec / recNode here; the records the view keeps are then compacted into the plan's rec / recNode.
+struct ViewScratch {
+    const uint8_t* drawn;         // [node index] 1 when kernel_render draws the node (simlod_export_view_flags)
+    SimlodExportNode* rec;        // [record] breadth-first records of every reachable node
+    uint32_t* recNode;            // [record] their node indices
+    uint8_t* mark;                // [record] 1 when a drawn record lies strictly below
+    uint32_t* index;              // [record] position among the kept records
+};
+static_assert(sizeof(ViewScratch) == 40, "ViewScratch");
+
+struct QueryCtl {                         // simlod_export_collect sees the ExportCtl it begins with
+    ExportCtl plan;                       // records, candidate samples (those of the visited nodes), items, error
+    uint64_t outSamples, outPoints, outVoxels;
+    uint32_t nodesVisited, pad;
+};
+static_assert(sizeof(QueryCtl) == 80 && offsetof(QueryCtl, plan) == 0 && offsetof(QueryCtl, outSamples) == 48, "QueryCtl");
+
+struct QueryBox { float mn[3], mx[3]; };  // boxMin / boxMax of the uniforms
+static_assert(sizeof(QueryBox) == 24, "QueryBox");
+
+// ---- octree import (import.cu) ------------------------------------------------------------------------------------
+
+enum : uint32_t {                         // the import's error word
+    IMPORT_ERR_POINT = 1,                 // a point whose descent does not end in its leaf
+    IMPORT_ERR_VOXEL = 2,                 // a voxel that is not the centre of a cell of its node
+    IMPORT_ERR_DUPLICATE = 4,             // two voxels in one cell of a node
+    IMPORT_ERR_COUNT = 8,                 // a node's voxels are not as many as the cells its points occupy
+};
+
+struct ImportPlan {                       // per record; one more entry after the last record (chunk = total)
+    uint64_t grid;                        // heap offset of the node's grid (0: none)
+    uint64_t chunk;                       // index of its first chunk: points first, then voxels
+    uint32_t row;                         // its chunk row (+1; 0: none)
+    uint32_t counter;                     // Node::counter from the file
+};
+static_assert(sizeof(ImportPlan) == 24, "ImportPlan");
+
+struct ImportArgs {
+    SimlodNode* nodes;
+    uint8_t* heap;
+    uint8_t* scratch;                     // kernel_construct's momentary buffer
+    const SimlodExportNode* rec;
+    const ImportPlan* plan;
+    uint32_t* error;
+    uint64_t chunkBase;                   // heap offset of chunk 0
+    uint32_t numRecords, numRows;
+    float boxMin[3], boxMax[3];
+};
+static_assert(sizeof(ImportArgs) == 88 && offsetof(ImportArgs, chunkBase) == 48 && offsetof(ImportArgs, boxMin) == 64, "ImportArgs");
+
+// ---- spatial exchange and depth compositing (partition.cu) --------------------------------------------------------
+
+namespace part {
+constexpr uint32_t MAX_RANKS = 8;
+constexpr uint32_t MAX_CELLS = 512;       // level <= 3
+constexpr uint32_t BLOCK = 256;           // threads per block of every partition kernel
+}  // namespace part
+
+struct PartitionParams {
+    float minx, miny, minz, size;           // octree cube: boxMin + max extent (voxels.cu:860-863)
+    uint32_t level;                         // 1..3
+    uint32_t numRanks;                      // 1..8
+    uint32_t count;
+    uint32_t perBlock;                      // points per block, a multiple of BLOCK
+    uint8_t owner[part::MAX_CELLS];         // cell (Morton order: child index per level, root first) -> rank
+};
+static_assert(sizeof(PartitionParams) == 544 && offsetof(PartitionParams, owner) == 32, "PartitionParams");
+
+struct ScatterTargets {
+    uint64_t ptr[part::MAX_RANKS];          // destination buffers (device addresses, local or peer)
+    uint64_t offset[part::MAX_RANKS];       // first point slot of THIS sender in each destination
+    uint64_t signal[part::MAX_RANKS];       // this sender's flag word in each destination (0 = no signalling)
+    uint32_t signalValue;
+    uint32_t pad;
+};
+static_assert(sizeof(ScatterTargets) == 200 && offsetof(ScatterTargets, signalValue) == 192, "ScatterTargets");
+
+struct CompositeArgs {
+    uint64_t fb[part::MAX_RANKS];           // every rank's framebuffer copy (device addresses, local or peer)
+    uint64_t signal[part::MAX_RANKS];
+    uint64_t numWords;
+    uint32_t numRanks, rank, signalValue, pad;
+};
+static_assert(sizeof(CompositeArgs) == 152 && offsetof(CompositeArgs, numWords) == 128, "CompositeArgs");
+
+struct SignalArgs { uint64_t signal[part::MAX_RANKS]; uint32_t numRanks, value; };
+static_assert(sizeof(SignalArgs) == 72 && offsetof(SignalArgs, numRanks) == 64, "SignalArgs");

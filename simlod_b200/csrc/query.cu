@@ -22,14 +22,6 @@
 #include "export_common.cuh"
 #include "region.cuh"
 
-struct QueryCtl {                         // mirrors host.cpp; simlod_export_collect sees the ExportCtl it begins with
-    ExportCtl plan;                       // records, candidate samples (those of the visited nodes), items, error
-    uint64_t outSamples, outPoints, outVoxels;
-    uint32_t nodesVisited, pad;
-};
-
-struct QueryBox { float mn[3], mx[3]; };  // boxMin / boxMax of the uniforms
-
 constexpr uint64_t VOXEL_ITEM = 1ull << 63;   // item word: count (after the scan: destination offset) | VOXEL_ITEM
 
 // Whether no eligible sample stored in a node with box `b` can pass the point predicate of `r`. Conservative: `false` is
