@@ -244,6 +244,42 @@ SIMLOD_STATIC_ASSERT(offsetof(SimlodQueryInfo, samples_tested) == 24 && offsetof
 int simlod_query_region(SimlodContext* ctx, const SimlodRegion* region, int32_t depth, uint64_t dst_samples,
                         uint64_t sample_capacity, SimlodQueryInfo* info, float* kernel_ms);
 
+// Pick (DESIGN.md §9.9): which stored sample each pixel of the frame simlod_render draws for the current uniforms shows, as
+// an index into the sample array simlod_export_view returns for the same uniforms (its records say which node holds the
+// sample and whether it is a point or a voxel).
+typedef struct SimlodPickInfo {
+    uint64_t num_hits;                              //   0  requested pixels that show a sample
+    uint64_t num_samples;                           //   8  samples of the view export: the index space
+    uint32_t num_nodes;                             //  16  records of the view export
+    uint32_t num_pixels;                            //  20  pixels requested
+    float    plan_ms, key_ms, index_ms, write_ms;   //  24  event time of each stage: the view's plan, the key pass (with
+                                                    //      the clear), the index pass, the write
+} SimlodPickInfo;
+SIMLOD_STATIC_ASSERT(sizeof(SimlodPickInfo) == 40, "PickInfo");
+SIMLOD_STATIC_ASSERT(offsetof(SimlodPickInfo, num_nodes) == 16 && offsetof(SimlodPickInfo, plan_ms) == 24, "PickInfo.num_nodes");
+//   candidates   every sample S[i] of the view export, projected as kernel_render projects it (pixel (x, y), depth w,
+//                inside); a candidate when inside and, with useHighQualityShading, depth > 0. Its key is
+//                k = float_bits(depth) << 32 | c, c the colour the frame displays (its own, by node or by level)
+//   pixels       a candidate covers clamp(x+ox, 0, W) + W * clamp(y+oy, 0, H) for 0 <= ox, oy < pointSize (W x H the
+//                context's frame); ids >= W*H are dropped, an id with x+ox == W wraps into the next row as in the frame
+//   winner       of a pixel: the covering candidate with the smallest (k, i). The pixel is hit when k < 0x7f800000_00332211
+//                (the frame's clear value), with useHighQualityShading when depth bits < 0x7f800000; never with
+//                showPoints == 0. The bounding-box overlay is not part of the result.
+// So after simlod_render with the same uniforms (showBoundingBox 0, a cut within the renderer's item capacity), a pixel
+// is -1 exactly where the framebuffer holds the clear value, and otherwise the framebuffer holds the winner's key (its
+// depth alone with useHighQualityShading) — before eye-dome lighting replaces the colour word of the pixels it shades.
+//   pixels == NULL     the whole frame, pixel p = x + W * y at dst_index[p] (num_pixels must be 0)
+//   pixels != NULL     num_pixels (x, y) pairs with x < W and y < H, 1 <= num_pixels <= W * H; pixel t at dst_index[t]
+// dst_index (int64, 8-byte aligned): the index, or -1. dst_samples (optional, 16-byte aligned): the picked SimlodPoint,
+// zeros where the index is -1. Both 0: *info only. SIMLOD_ERR_INVALID before any launch, with nothing written, for a
+// pixel outside the frame, an empty or oversized list or a misaligned destination; after the plan, with nothing
+// written, for an inconsistent image (the export's conditions). Writes nothing into the context's buffers or Stats
+// (not even Node::visible / isLarge); two picks of the same state are byte-identical. Enqueued on the launch stream;
+// returns once complete. *kernel_ms (optional) = event time of all its kernels. Scratch: two W x H u64 frames and the
+// pixel list, kept until simlod_destroy, besides the export's.
+int simlod_pick(SimlodContext* ctx, const uint32_t* pixels, uint64_t num_pixels, uint64_t dst_index, uint64_t dst_samples,
+                SimlodPickInfo* info, float* kernel_ms);
+
 // Octree files (SimlodOctreeFileHeader, DESIGN.md §9.7): a built octree saved and loaded back, so that it can be rendered,
 // exported or continued with new batches in another context, process or session.
 // simlod_read_octree_header: the header of an octree file, checked against itself and the file size. No context, no GPU.

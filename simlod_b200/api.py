@@ -150,6 +150,13 @@ class SimlodQueryInfo(C.Structure):
                 ("nodes_visited", C.c_uint32), ("max_level", C.c_uint32)]
 
 
+class SimlodPickInfo(C.Structure):
+    """SimlodPickInfo: hits among the requested pixels, the view export's sample and record counts (the index space), and
+    the event time of each stage of the pick."""
+    _fields_ = [("num_hits", C.c_uint64), ("num_samples", C.c_uint64), ("num_nodes", C.c_uint32), ("num_pixels", C.c_uint32),
+                ("plan_ms", C.c_float), ("key_ms", C.c_float), ("index_ms", C.c_float), ("write_ms", C.c_float)]
+
+
 class Region:
     """Constructors of the regions SimLOD.query_region takes. Numbers are rounded to float32, the type the predicates are
     evaluated in; a malformed region (non-finite number, min > max, negative radius) is refused by the query."""
@@ -194,6 +201,7 @@ assert C.sizeof(ExportInfo) == 32 and EXPORT_NODE_DTYPE.itemsize == 64
 assert C.sizeof(LasHeader) == 128
 assert C.sizeof(OctreeFileHeader) == 128
 assert C.sizeof(SimlodRegion) == 304 and C.sizeof(SimlodQueryInfo) == 40
+assert C.sizeof(SimlodPickInfo) == 40
 
 # every symbol include/simlod_b200.h declares
 EXPORTS = [
@@ -207,6 +215,7 @@ EXPORTS = [
     "simlod_export_framebuffer", "simlod_peer_signal", "simlod_composite_framebuffers", "simlod_generate", "simlod_reset_with_grid", "simlod_insert_simlod_file_ex", "simlod_get_numa_node",
     "simlod_export_octree", "simlod_export_view", "simlod_read_las_header", "simlod_insert_files",
     "simlod_read_octree_header", "simlod_save_octree", "simlod_load_octree", "simlod_query_region",
+    "simlod_pick",
 ]
 
 _lib = None
@@ -270,6 +279,7 @@ def load_library():
         "simlod_save_octree": [vp, C.c_char_p, C.POINTER(ExportInfo), C.POINTER(C.c_float)],
         "simlod_load_octree": [vp, C.c_char_p, C.c_int, C.POINTER(ExportInfo), C.POINTER(C.c_float)],
         "simlod_query_region": [vp, C.POINTER(SimlodRegion), C.c_int32, u64, u64, C.POINTER(SimlodQueryInfo), C.POINTER(C.c_float)],
+        "simlod_pick": [vp, C.POINTER(C.c_uint32), u64, u64, u64, C.POINTER(SimlodPickInfo), C.POINTER(C.c_float)],
     }
     for name, argtypes in sig.items():
         fn = getattr(lib, name)
@@ -667,6 +677,59 @@ class SimLOD:
         if m:
             info, _ = self.query_region_into(region, depth, samples.data_ptr(), m)
         return samples, info
+
+    def pick_into(self, pixels, dst_index, dst_samples):
+        """simlod_pick into caller-owned device memory: pixels None for the whole frame, else an (N, 2) array of (x, y);
+        dst_index (int64) and dst_samples (16-byte samples, 0 for none) both 0: info only. Returns (SimlodPickInfo,
+        kernel ms)."""
+        info, ms = SimlodPickInfo(), C.c_float(0)
+        if pixels is None:
+            ptr, n = None, 0
+        else:
+            a = np.asarray(pixels)
+            if a.ndim != 2 or a.shape[1] != 2 or (a.size and a.dtype.kind not in "iu"):
+                raise ValueError("pixels must be an (N, 2) integer array of (x, y)")
+            a = a.astype(np.int64)
+            # negative or huge coordinates become ones the library refuses as outside the frame
+            a = np.ascontiguousarray(np.where((a < 0) | (a > 0xFFFFFFFF), 0xFFFFFFFF, a).astype(np.uint32))
+            n = a.shape[0]
+            keep = a if n else np.zeros(2, dtype=np.uint32)        # an empty list is still a list (and is refused)
+            ptr = keep.ctypes.data_as(C.POINTER(C.c_uint32))
+        self._check(self._lib.simlod_pick(self._ctx, ptr, n, int(dst_index), int(dst_samples), C.byref(info), C.byref(ms)))
+        return info, ms.value
+
+    def pick(self, pixels=None, device="cuda", samples=False):
+        """The sample under each pixel of the frame render() draws for the current uniforms (simlod_pick): an index into
+        export_view().samples, -1 where the frame shows no sample. pixels=None picks the whole frame, an (H, W) int64
+        result; an (N, 2) array of (x, y) with x < width and y < height picks those pixels, an (N,) result. With
+        samples=True the picked samples are returned too, (H, W, 4) or (N, 4) float32 in the export's layout (x, y, z,
+        colour bits), zeros where the index is -1. device="cuda": torch tensors in device memory; device="cpu": numpy
+        arrays (the samples as POINT_DTYPE). Returns (index, info) or, with samples=True, (index, samples, info)."""
+        shape = (self.height, self.width) if pixels is None else (len(np.asarray(pixels)),)
+        n = int(np.prod(shape))
+        if device == "cpu":
+            di = self.device_alloc(max(n, 1) * 8)
+            ds = self.device_alloc(max(n, 1) * 16) if samples else 0
+            try:
+                info, _ = self.pick_into(pixels, di, ds)
+                index = self.memcpy_dtoh(di, n * 8).view(np.int64).reshape(shape)
+                picked = self.memcpy_dtoh(ds, n * 16).view(POINT_DTYPE).reshape(shape) if samples else None
+            finally:
+                self.device_free(di)
+                if ds:
+                    self.device_free(ds)
+            return (index, picked, info) if samples else (index, info)
+        import torch
+        dev = torch.device(device)
+        if dev.type != "cuda":
+            raise ValueError("device must be 'cpu' or a CUDA device, not %r" % device)
+        if dev.index is None:
+            dev = torch.device("cuda", self.device)
+        index = torch.empty(shape, dtype=torch.int64, device=dev)
+        picked = torch.empty(shape + (4,), dtype=torch.float32, device=dev) if samples else None
+        torch.cuda.current_stream(dev).synchronize()       # the caching allocator may hand out memory torch still uses
+        info, _ = self.pick_into(pixels, index.data_ptr() if n else 0, picked.data_ptr() if samples and n else 0)
+        return (index, picked, info) if samples else (index, info)
 
     def host_alloc(self, nbytes):
         p = C.c_void_p()

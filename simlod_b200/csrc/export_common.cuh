@@ -12,6 +12,17 @@ struct Item { uint64_t src; uint64_t dst; };   // dst: sample index | count << 4
 
 __device__ __forceinline__ uint32_t ceilChunks(uint32_t n) { return (n + PPC - 1) / PPC; }
 
+// The record that chunk item k belongs to: the last one whose first item is <= k (recItem is non-decreasing; records
+// without items share a value with the next record)
+__device__ __forceinline__ uint32_t itemRecord(uint64_t k, const uint64_t* __restrict__ recItem, uint32_t n) {
+    uint32_t lo = 0, hi = n;               // recItem[lo] <= k < recItem[hi] (recItem[n] = numItems)
+    while (hi - lo > 1) {
+        const uint32_t mid = (lo + hi) >> 1;
+        if (recItem[mid] <= k) lo = mid; else hi = mid;
+    }
+    return lo;
+}
+
 // Block-wide exclusive scan (PLAN_THREADS threads) of 64-bit values; returns the prefix, *total the sum. One instance per
 // plan kernel (isView), so that each kernel has its own warpSums and the full / depth plan keeps its shared-memory layout.
 template <bool isView>

@@ -48,6 +48,7 @@ extern const unsigned char simlod_cubin_gen[];
 extern const unsigned char simlod_cubin_export[];
 extern const unsigned char simlod_cubin_import[];
 extern const unsigned char simlod_cubin_query[];
+extern const unsigned char simlod_cubin_pick[];
 }
 
 namespace {
@@ -113,9 +114,9 @@ struct Program {
 
 // The embedded images of the kernels that are launched outside the three swappable programs, and those kernels: one
 // row each, {enum value, image, kernel name}. createResources loads every image and looks up every kernel.
-enum Image { IMG_UTIL, IMG_LAS, IMG_GEN, IMG_PARTITION, IMG_EXPORT, IMG_QUERY, IMG_IMPORT, NUM_IMAGES };
+enum Image { IMG_UTIL, IMG_LAS, IMG_GEN, IMG_PARTITION, IMG_EXPORT, IMG_QUERY, IMG_IMPORT, IMG_PICK, NUM_IMAGES };
 const unsigned char* const IMAGES[NUM_IMAGES] = {simlod_cubin_util, simlod_cubin_las, simlod_cubin_gen, simlod_cubin_partition,
-                                                 simlod_cubin_export, simlod_cubin_query, simlod_cubin_import};
+                                                 simlod_cubin_export, simlod_cubin_query, simlod_cubin_import, simlod_cubin_pick};
 #define KERNEL_LIST(X)                                                                                    \
     X(K_RCP, IMG_UTIL, "simlod_util_rcp") X(K_FILL, IMG_UTIL, "simlod_util_fill")                         \
     X(K_LAS, IMG_LAS, "simlod_las_decode")                                                                \
@@ -132,7 +133,9 @@ const unsigned char* const IMAGES[NUM_IMAGES] = {simlod_cubin_util, simlod_cubin
     X(K_QUERY_SCAN, IMG_QUERY, "simlod_query_scan") X(K_QUERY_WRITE, IMG_QUERY, "simlod_query_write")     \
     X(K_IMPORT_NODES, IMG_IMPORT, "simlod_import_nodes") X(K_IMPORT_LINK, IMG_IMPORT, "simlod_import_link") \
     X(K_IMPORT_CLEAR_GRIDS, IMG_IMPORT, "simlod_import_clear_grids") X(K_IMPORT_SCATTER, IMG_IMPORT, "simlod_import_scatter") \
-    X(K_IMPORT_VOXELS, IMG_IMPORT, "simlod_import_voxels") X(K_IMPORT_COUNT_GRIDS, IMG_IMPORT, "simlod_import_count_grids")
+    X(K_IMPORT_VOXELS, IMG_IMPORT, "simlod_import_voxels") X(K_IMPORT_COUNT_GRIDS, IMG_IMPORT, "simlod_import_count_grids") \
+    X(K_PICK_CLEAR, IMG_PICK, "simlod_pick_clear") X(K_PICK_KEY, IMG_PICK, "simlod_pick_key")             \
+    X(K_PICK_INDEX, IMG_PICK, "simlod_pick_index") X(K_PICK_WRITE, IMG_PICK, "simlod_pick_write")
 #define X(k, image, name) k,
 enum Kernel { KERNEL_LIST(X) NUM_KERNELS };
 #undef X
@@ -197,6 +200,8 @@ struct SimlodContext {
     CUdeviceptr exportScratch = 0;     // octree export and region query: see scratchFor()
     uint64_t exportScratchBytes = 0;
     void* hExportCtl = nullptr;        // pinned copy of ExportCtl / QueryCtl (CTL_HOST_BYTES)
+    CUdeviceptr pickScratch = 0;       // pick: key frame | index frame | hit counter | pixel list
+    uint64_t pickScratchBytes = 0;
     CUdeviceptr fileWindow = 0;        // octree files: FILE_WINDOW_BYTES of samples staged on the device
     CUdeviceptr fileTables = 0;        // octree load: records | plan | error word, sized for nodes[]
     uint64_t fileTablesBytes = 0;
@@ -612,6 +617,7 @@ void simlod_destroy(SimlodContext* ctx) {
         }
         if (ctx->exportScratch) D(cuMemFree)(ctx->exportScratch);
         if (ctx->hExportCtl) D(cuMemFreeHost)(ctx->hExportCtl);
+        if (ctx->pickScratch) D(cuMemFree)(ctx->pickScratch);
         if (ctx->fileWindow) D(cuMemFree)(ctx->fileWindow);
         if (ctx->fileTables) D(cuMemFree)(ctx->fileTables);
         delete ctx->loaderPool;          // joins the loader threads
@@ -1617,6 +1623,66 @@ int simlod_query_region(SimlodContext* ctx, const SimlodRegion* region, int32_t 
     float writeMs = 0.0f;
     CU(D(cuEventElapsedTime)(&writeMs, ctx->evTotalStart, ctx->evTotalEnd));
     if (kernel_ms) *kernel_ms = ms + writeMs;
+    return SIMLOD_OK;
+}
+
+// ---- pick (DESIGN.md §9.9); kernels in pick.cu, the plan is the view export's ------------------------------------------
+int simlod_pick(SimlodContext* ctx, const uint32_t* pixels, uint64_t num_pixels, uint64_t dst_index, uint64_t dst_samples,
+                SimlodPickInfo* info, float* kernel_ms) {
+    int rc = setCurrent(ctx); if (rc) return rc;
+    if (!info) return fail(SIMLOD_ERR_INVALID, "null info");
+    const uint32_t width = ctx->cfg.width, height = ctx->cfg.height;
+    const uint64_t frame = (uint64_t)width * height;
+    std::vector<uint32_t> ids;
+    if (pixels) {
+        if (num_pixels == 0 || num_pixels > frame)
+            return fail(SIMLOD_ERR_INVALID, "pixel list of %llu pixels, 1 to %llu (the frame) are supported", (unsigned long long)num_pixels, (unsigned long long)frame);
+        ids.resize(num_pixels);
+        for (uint64_t t = 0; t < num_pixels; t++) {
+            const uint32_t x = pixels[2 * t], y = pixels[2 * t + 1];
+            if (x >= width || y >= height)
+                return fail(SIMLOD_ERR_INVALID, "pixel %llu (%u, %u) lies outside the %ux%u frame", (unsigned long long)t, x, y, width, height);
+            ids[t] = x + width * y;
+        }
+    } else if (num_pixels) {
+        return fail(SIMLOD_ERR_INVALID, "num_pixels without a pixel list");
+    }
+    if (dst_index % 8 || dst_samples % 16) return fail(SIMLOD_ERR_INVALID, "pick destinations must be 8-byte (indices) and 16-byte (samples) aligned");
+    const uint32_t n = (uint32_t)(pixels ? num_pixels : frame);
+    // stage 1: the view export's plan, into its scratch, and the one host round trip for its control word
+    ExportPlanned p;
+    rc = exportPlan(ctx, -1, &ctx->uniforms, &p);
+    if (kernel_ms) *kernel_ms = p.ms;
+    if (rc) return rc;
+    // stage 2: the two frames, then the indices of the requested pixels
+    rc = growDevice(&ctx->pickScratch, &ctx->pickScratchBytes, 16 * frame + 16 + 4ull * n); if (rc) return rc;
+    const CUdeviceptr base = ctx->pickScratch, list = pixels ? base + 16 * frame + 16 : 0;
+    if (pixels) CU(D(cuMemcpyHtoDAsync)(list, ids.data(), 4ull * n, ctx->streamMain));
+    PickArgs a{devPtr(p.s.rec), devPtr(p.s.recItem), devPtr(p.s.items), devPtr(base), devPtr(base + 8 * frame), devPtr(base + 16 * frame),
+               p.c.numItems, p.c.numNodes, 0};
+    SimlodUniforms u = ctx->uniforms;
+    CUdeviceptr di = (CUdeviceptr)dst_index, ds = (CUdeviceptr)dst_samples;
+    uint32_t count = n;
+    const unsigned blocks = (unsigned)ctx->numSMs * 4;
+    CU(D(cuEventRecord)(ctx->evStart, ctx->streamMain));
+    rc = launch(ctx, ctx->fn[K_PICK_CLEAR], blocks, 256, ctx->streamMain, u, a); if (rc) return rc;
+    rc = launch(ctx, ctx->fn[K_PICK_KEY], blocks, 256, ctx->streamMain, u, a); if (rc) return rc;
+    CU(D(cuEventRecord)(ctx->evEnd, ctx->streamMain));
+    rc = launch(ctx, ctx->fn[K_PICK_INDEX], blocks, 256, ctx->streamMain, u, a); if (rc) return rc;
+    CU(D(cuEventRecord)(ctx->evTotalStart, ctx->streamMain));
+    rc = launch(ctx, ctx->fn[K_PICK_WRITE], blocks, 256, ctx->streamMain, a, list, count, di, ds); if (rc) return rc;
+    CU(D(cuEventRecord)(ctx->evTotalEnd, ctx->streamMain));
+    uint64_t hits = 0;
+    CU(D(cuMemcpyDtoHAsync)(ctx->hExportCtl, base + 16 * frame, 8, ctx->streamMain));
+    CU(D(cuStreamSynchronize)(ctx->streamMain));
+    memcpy(&hits, ctx->hExportCtl, 8);
+    float keyMs = 0.0f, indexMs = 0.0f, writeMs = 0.0f;
+    CU(D(cuEventElapsedTime)(&keyMs, ctx->evStart, ctx->evEnd));
+    CU(D(cuEventElapsedTime)(&indexMs, ctx->evEnd, ctx->evTotalStart));
+    CU(D(cuEventElapsedTime)(&writeMs, ctx->evTotalStart, ctx->evTotalEnd));
+    info->num_hits = hits; info->num_samples = p.c.numSamples; info->num_nodes = p.c.numNodes; info->num_pixels = n;
+    info->plan_ms = p.ms; info->key_ms = keyMs; info->index_ms = indexMs; info->write_ms = writeMs;
+    if (kernel_ms) *kernel_ms = p.ms + keyMs + indexMs + writeMs;
     return SIMLOD_OK;
 }
 

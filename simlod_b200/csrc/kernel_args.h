@@ -1,6 +1,6 @@
 // kernel_args.h — the argument and control structs that host.cpp fills and the kernels read, with the codes and limits
 // both sides use. One definition for both compilers: plain C++ (no device code), included by host.cpp and by export.cu,
-// query.cu (through export_common.cuh), import.cu and partition.cu. The static_asserts pin every size, and the offsets
+// query.cu and pick.cu (through export_common.cuh), import.cu and partition.cu. The static_asserts pin every size, and the offsets
 // that one side reads of a struct the other writes, so a layout change fails to compile instead of shifting bytes.
 #pragma once
 #include <stddef.h>
@@ -44,6 +44,20 @@ static_assert(sizeof(QueryCtl) == 80 && offsetof(QueryCtl, plan) == 0 && offseto
 
 struct QueryBox { float mn[3], mx[3]; };  // boxMin / boxMax of the uniforms
 static_assert(sizeof(QueryBox) == 24, "QueryBox");
+
+// ---- pick (pick.cu) -------------------------------------------------------------------------------------------------
+
+struct PickArgs {                         // the view export's plan (export scratch) and the pick's two frames
+    const SimlodExportNode* rec;          // [record] the view's records
+    const uint64_t* recItem;              // [record] its first chunk item
+    const uint64_t* items;                // [item] two words: Item {src, dst | count << 48} (export_common.cuh)
+    uint64_t* key;                        // [pixel] smallest candidate key depth << 32 | colour
+    uint64_t* index;                      // [pixel] smallest sample index with that key, ~0 for none
+    uint64_t* hits;                       // picked pixels among those the write kernel visits
+    uint64_t numItems;
+    uint32_t numRecords, pad;
+};
+static_assert(sizeof(PickArgs) == 64 && offsetof(PickArgs, numItems) == 48, "PickArgs");
 
 // ---- octree import (import.cu) ------------------------------------------------------------------------------------
 

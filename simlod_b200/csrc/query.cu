@@ -210,15 +210,10 @@ __device__ __forceinline__ uint32_t filterItem(const uint4* __restrict__ src, ui
     return passed;
 }
 
-// Whether item k holds voxels: the items of a record are those of its point list, then those of its voxel list. The
-// record is the last one whose first item is <= k (recItem is non-decreasing; records without items share a value).
+// Whether item k holds voxels: the items of a record are those of its point list, then those of its voxel list.
 __device__ __forceinline__ bool itemIsVoxel(uint64_t k, const SimlodExportNode* __restrict__ rec, const uint64_t* __restrict__ recItem, uint32_t n) {
-    uint32_t lo = 0, hi = n;               // recItem[lo] <= k < recItem[hi] (recItem[n] = numItems)
-    while (hi - lo > 1) {
-        const uint32_t mid = (lo + hi) >> 1;
-        if (recItem[mid] <= k) lo = mid; else hi = mid;
-    }
-    return k - recItem[lo] >= ceilChunks(rec[lo].num_points);
+    const uint32_t r = itemRecord(k, recItem, n);
+    return k - recItem[r] >= ceilChunks(rec[r].num_points);
 }
 
 extern "C" __global__ void __launch_bounds__(256)
