@@ -280,6 +280,48 @@ SIMLOD_STATIC_ASSERT(offsetof(SimlodPickInfo, num_nodes) == 16 && offsetof(Simlo
 int simlod_pick(SimlodContext* ctx, const uint32_t* pixels, uint64_t num_pixels, uint64_t dst_index, uint64_t dst_samples,
                 SimlodPickInfo* info, float* kernel_ms);
 
+// k nearest samples (DESIGN.md §9.10): for each query position, the k samples of a sample set with the smallest key, as
+// indices into the sample array simlod_export_octree(depth) returns for the same state (its records say which node holds
+// a sample and whether it is a point or a voxel).
+#define SIMLOD_NEAREST_MAX_K 32
+#define SIMLOD_NEAREST_MAX_QUERIES (1u << 24)
+typedef struct SimlodNearestInfo {
+    uint64_t num_samples;                           //   0  samples of the export at `depth`: the index space
+    uint64_t num_found;                             //   8  filled slots, summed over the queries
+    uint64_t samples_tested;                        //  16  distance evaluations, summed over the queries
+    uint64_t records_visited;                       //  24  records whose samples were evaluated, summed over the queries
+    uint32_t num_queries, k;                        //  32
+    uint32_t invalid_queries;                       //  40  queries with a non-finite coordinate (k empty slots each)
+    uint32_t max_level;                             //  44  deepest level in the octree
+    float    plan_ms, bucket_ms, search_ms;         //  48  event time of the export's plan, of the locate + bucketing, and of
+                                                    //      the search (which writes the destinations)
+    uint32_t reserved;                              //  60
+} SimlodNearestInfo;
+SIMLOD_STATIC_ASSERT(sizeof(SimlodNearestInfo) == 64, "NearestInfo");
+SIMLOD_STATIC_ASSERT(offsetof(SimlodNearestInfo, num_queries) == 32 && offsetof(SimlodNearestInfo, plan_ms) == 48, "NearestInfo.num_queries");
+//   sample set   as simlod_query_region's: depth < 0, the eligible points of every leaf (the inserted point set);
+//                0 <= depth <= 20, the export's cut at `depth`, its points eligible ones, its voxels always
+//   key          of sample p for query q: d = p - q per coordinate, d2 = (dx*dx + dy*dy) + dz*dz in float32 without
+//                contraction (the sphere predicate's sequence); samples are ordered by (d2, index). d2 may be +inf.
+//   candidates   the samples of the set with d2 <= max_radius * max_radius (float32); max_radius = +inf for no limit
+//   result       k slots per query in ascending key order: dst_index[q][j] (int64), dst_dist2[q][j] (float32) and
+//                dst_samples[q][j] (the 16-byte SimlodPoint, bit for bit export_octree(depth).samples[index]). A slot
+//                beyond the candidates is empty: index -1, d2 +inf, sample all zero. A query with a non-finite coordinate
+//                gets k empty slots and counts in info->invalid_queries.
+//   queries      a device address of num_queries 16-byte records (x, y, z, one ignored word), 16-byte aligned, so the
+//                samples of an export, a region query or a pick can be passed as they are; queries may lie outside the cube
+// Each destination may be 0 (not written). SIMLOD_ERR_INVALID before any launch, with nothing written, for k outside
+// 1..SIMLOD_NEAREST_MAX_K, num_queries 0 or above SIMLOD_NEAREST_MAX_QUERIES, depth > 20, a NaN or negative
+// max_radius, a null or misaligned query array or a misaligned destination; with nothing written, for an inconsistent
+// image (the export's conditions, and a record tree whose levels do not step by one from the root to at most 20). A
+// record whose lattice box cannot hold a candidate that beats a query's k-th key is skipped unread, so the result
+// equals an exhaustive search, and two calls on the same state are byte-identical. Reads the ABI only, as the export
+// does, and writes nothing into the context's buffers or Stats. Enqueued on the launch stream; returns once complete.
+// *kernel_ms (optional) = event time of all its kernels. Scratch: the export's, and 12 bytes per query and 12 per record,
+// kept until simlod_destroy.
+int simlod_query_nearest(SimlodContext* ctx, uint64_t queries, uint64_t num_queries, uint32_t k, int32_t depth, float max_radius,
+                         uint64_t dst_index, uint64_t dst_dist2, uint64_t dst_samples, SimlodNearestInfo* info, float* kernel_ms);
+
 // Octree files (SimlodOctreeFileHeader, DESIGN.md §9.7): a built octree saved and loaded back, so that it can be rendered,
 // exported or continued with new batches in another context, process or session.
 // simlod_read_octree_header: the header of an octree file, checked against itself and the file size. No context, no GPU.

@@ -157,6 +157,19 @@ class SimlodPickInfo(C.Structure):
                 ("plan_ms", C.c_float), ("key_ms", C.c_float), ("index_ms", C.c_float), ("write_ms", C.c_float)]
 
 
+NEAREST_MAX_K = 32
+NEAREST_MAX_QUERIES = 1 << 24
+
+
+class SimlodNearestInfo(C.Structure):
+    """SimlodNearestInfo: the export's sample count (the index space), filled slots, how much of the octree the search
+    had to look at, and the event time of each stage."""
+    _fields_ = [("num_samples", C.c_uint64), ("num_found", C.c_uint64), ("samples_tested", C.c_uint64),
+                ("records_visited", C.c_uint64), ("num_queries", C.c_uint32), ("k", C.c_uint32), ("invalid_queries", C.c_uint32),
+                ("max_level", C.c_uint32), ("plan_ms", C.c_float), ("bucket_ms", C.c_float), ("search_ms", C.c_float),
+                ("reserved", C.c_uint32)]
+
+
 class Region:
     """Constructors of the regions SimLOD.query_region takes. Numbers are rounded to float32, the type the predicates are
     evaluated in; a malformed region (non-finite number, min > max, negative radius) is refused by the query."""
@@ -201,7 +214,7 @@ assert C.sizeof(ExportInfo) == 32 and EXPORT_NODE_DTYPE.itemsize == 64
 assert C.sizeof(LasHeader) == 128
 assert C.sizeof(OctreeFileHeader) == 128
 assert C.sizeof(SimlodRegion) == 304 and C.sizeof(SimlodQueryInfo) == 40
-assert C.sizeof(SimlodPickInfo) == 40
+assert C.sizeof(SimlodPickInfo) == 40 and C.sizeof(SimlodNearestInfo) == 64
 
 # every symbol include/simlod_b200.h declares
 EXPORTS = [
@@ -215,7 +228,7 @@ EXPORTS = [
     "simlod_export_framebuffer", "simlod_peer_signal", "simlod_composite_framebuffers", "simlod_generate", "simlod_reset_with_grid", "simlod_insert_simlod_file_ex", "simlod_get_numa_node",
     "simlod_export_octree", "simlod_export_view", "simlod_read_las_header", "simlod_insert_files",
     "simlod_read_octree_header", "simlod_save_octree", "simlod_load_octree", "simlod_query_region",
-    "simlod_pick",
+    "simlod_pick", "simlod_query_nearest",
 ]
 
 _lib = None
@@ -280,6 +293,8 @@ def load_library():
         "simlod_load_octree": [vp, C.c_char_p, C.c_int, C.POINTER(ExportInfo), C.POINTER(C.c_float)],
         "simlod_query_region": [vp, C.POINTER(SimlodRegion), C.c_int32, u64, u64, C.POINTER(SimlodQueryInfo), C.POINTER(C.c_float)],
         "simlod_pick": [vp, C.POINTER(C.c_uint32), u64, u64, u64, C.POINTER(SimlodPickInfo), C.POINTER(C.c_float)],
+        "simlod_query_nearest": [vp, u64, u64, u32, C.c_int32, C.c_float, u64, u64, u64, C.POINTER(SimlodNearestInfo),
+                                 C.POINTER(C.c_float)],
     }
     for name, argtypes in sig.items():
         fn = getattr(lib, name)
@@ -730,6 +745,80 @@ class SimLOD:
         torch.cuda.current_stream(dev).synchronize()       # the caching allocator may hand out memory torch still uses
         info, _ = self.pick_into(pixels, index.data_ptr() if n else 0, picked.data_ptr() if samples and n else 0)
         return (index, picked, info) if samples else (index, info)
+
+    def query_nearest_into(self, queries_ptr, n, k, depth, max_radius, dst_index, dst_dist2, dst_samples):
+        """simlod_query_nearest on caller-owned device memory: n 16-byte query records at queries_ptr, destinations
+        [n][k] int64 / float32 / 16-byte samples, each 0 for not written (depth None or < 0: the inserted points;
+        max_radius None: no limit). Returns (SimlodNearestInfo, kernel ms)."""
+        info, ms = SimlodNearestInfo(), C.c_float(0)
+        d = -1 if depth is None else int(depth)
+        r = float("inf") if max_radius is None else float(max_radius)
+        self._check(self._lib.simlod_query_nearest(self._ctx, int(queries_ptr), int(n), int(k), d, r, int(dst_index),
+                                                   int(dst_dist2), int(dst_samples), C.byref(info), C.byref(ms)))
+        return info, ms.value
+
+    def query_nearest(self, queries, k=8, depth=None, max_radius=None, device="cuda", samples=False):
+        """The k nearest samples of each query position (simlod_query_nearest), exact: with depth=None among the
+        inserted points (those on the cube's max face excepted, as query_region), with an integer depth among the
+        samples of export_octree(depth). Samples are ordered by squared distance in float32, ties by index, and only
+        those within max_radius count. `queries`: an (N, 3) or (N, 4) array (the 4th column is ignored), numpy or a CUDA
+        tensor, or POINT_DTYPE samples. Returns (index, dist2, info) or, with samples=True, (index, dist2, samples, info):
+        (N, k) int64 indices into export_octree(depth).samples, -1 in an empty slot; (N, k) float32 squared distances,
+        +inf in an empty slot; (N, k, 4) float32 samples in the export's layout, zeros in an empty slot. device="cuda":
+        torch tensors in device memory; device="cpu": numpy arrays (the samples as POINT_DTYPE)."""
+        if isinstance(queries, np.ndarray) and queries.dtype == POINT_DTYPE:
+            queries = queries.view(np.float32).reshape(-1, 4)
+        if not isinstance(queries, np.ndarray) and hasattr(queries, "data_ptr"):
+            import torch
+            if not queries.is_cuda or queries.ndim != 2 or queries.shape[1] not in (3, 4):
+                raise ValueError("queries must be an (N, 3) or (N, 4) CUDA tensor or numpy array")
+            q = queries.detach().to(torch.float32)
+            if q.shape[1] == 3 or not q.is_contiguous() or q.data_ptr() % 16:
+                q4 = torch.zeros((q.shape[0], 4), dtype=torch.float32, device=q.device)
+                q4[:, :3] = q[:, :3]
+                q = q4
+            torch.cuda.current_stream(q.device).synchronize()  # the queries may still be being computed on torch's stream
+            return self._nearest(q.data_ptr(), q.shape[0], k, depth, max_radius, device, samples, keep=q)
+        a = np.asarray(queries)
+        if a.ndim != 2 or a.shape[1] not in (3, 4):
+            raise ValueError("queries must be an (N, 3) or (N, 4) CUDA tensor or numpy array")
+        q = np.zeros((a.shape[0], 4), dtype=np.float32)
+        q[:, :3] = a[:, :3]
+        dq = self.device_alloc(max(q.nbytes, 16))
+        try:
+            self.memcpy_htod(dq, q)
+            return self._nearest(dq, q.shape[0], k, depth, max_radius, device, samples)
+        finally:
+            self.device_free(dq)
+
+    def _nearest(self, qptr, n, k, depth, max_radius, device, samples, keep=None):
+        if device == "cpu":
+            m = max(n * k, 1)
+            di, dd = self.device_alloc(m * 8), self.device_alloc(m * 4)
+            ds = self.device_alloc(m * 16) if samples else 0
+            try:
+                info, _ = self.query_nearest_into(qptr, n, k, depth, max_radius, di, dd, ds)
+                index = self.memcpy_dtoh(di, n * k * 8).view(np.int64).reshape(n, k)
+                dist2 = self.memcpy_dtoh(dd, n * k * 4).view(np.float32).reshape(n, k)
+                found = self.memcpy_dtoh(ds, n * k * 16).view(POINT_DTYPE).reshape(n, k) if samples else None
+            finally:
+                for p in (di, dd, ds):
+                    if p:
+                        self.device_free(p)
+            return (index, dist2, found, info) if samples else (index, dist2, info)
+        import torch
+        dev = torch.device(device)
+        if dev.type != "cuda":
+            raise ValueError("device must be 'cpu' or a CUDA device, not %r" % device)
+        if dev.index is None:
+            dev = torch.device("cuda", self.device)
+        index = torch.empty((n, k), dtype=torch.int64, device=dev)
+        dist2 = torch.empty((n, k), dtype=torch.float32, device=dev)
+        found = torch.empty((n, k, 4), dtype=torch.float32, device=dev) if samples else None
+        torch.cuda.current_stream(dev).synchronize()       # the caching allocator may hand out memory torch still uses
+        info, _ = self.query_nearest_into(qptr, n, k, depth, max_radius, index.data_ptr() if n else 0,
+                                          dist2.data_ptr() if n else 0, found.data_ptr() if samples and n else 0)
+        return (index, dist2, found, info) if samples else (index, dist2, info)
 
     def host_alloc(self, nbytes):
         p = C.c_void_p()

@@ -49,6 +49,7 @@ extern const unsigned char simlod_cubin_export[];
 extern const unsigned char simlod_cubin_import[];
 extern const unsigned char simlod_cubin_query[];
 extern const unsigned char simlod_cubin_pick[];
+extern const unsigned char simlod_cubin_nearest[];
 }
 
 namespace {
@@ -114,9 +115,10 @@ struct Program {
 
 // The embedded images of the kernels that are launched outside the three swappable programs, and those kernels: one
 // row each, {enum value, image, kernel name}. createResources loads every image and looks up every kernel.
-enum Image { IMG_UTIL, IMG_LAS, IMG_GEN, IMG_PARTITION, IMG_EXPORT, IMG_QUERY, IMG_IMPORT, IMG_PICK, NUM_IMAGES };
+enum Image { IMG_UTIL, IMG_LAS, IMG_GEN, IMG_PARTITION, IMG_EXPORT, IMG_QUERY, IMG_IMPORT, IMG_PICK, IMG_NEAREST, NUM_IMAGES };
 const unsigned char* const IMAGES[NUM_IMAGES] = {simlod_cubin_util, simlod_cubin_las, simlod_cubin_gen, simlod_cubin_partition,
-                                                 simlod_cubin_export, simlod_cubin_query, simlod_cubin_import, simlod_cubin_pick};
+                                                 simlod_cubin_export, simlod_cubin_query, simlod_cubin_import, simlod_cubin_pick,
+                                                 simlod_cubin_nearest};
 #define KERNEL_LIST(X)                                                                                    \
     X(K_RCP, IMG_UTIL, "simlod_util_rcp") X(K_FILL, IMG_UTIL, "simlod_util_fill")                         \
     X(K_LAS, IMG_LAS, "simlod_las_decode")                                                                \
@@ -135,7 +137,9 @@ const unsigned char* const IMAGES[NUM_IMAGES] = {simlod_cubin_util, simlod_cubin
     X(K_IMPORT_CLEAR_GRIDS, IMG_IMPORT, "simlod_import_clear_grids") X(K_IMPORT_SCATTER, IMG_IMPORT, "simlod_import_scatter") \
     X(K_IMPORT_VOXELS, IMG_IMPORT, "simlod_import_voxels") X(K_IMPORT_COUNT_GRIDS, IMG_IMPORT, "simlod_import_count_grids") \
     X(K_PICK_CLEAR, IMG_PICK, "simlod_pick_clear") X(K_PICK_KEY, IMG_PICK, "simlod_pick_key")             \
-    X(K_PICK_INDEX, IMG_PICK, "simlod_pick_index") X(K_PICK_WRITE, IMG_PICK, "simlod_pick_write")
+    X(K_PICK_INDEX, IMG_PICK, "simlod_pick_index") X(K_PICK_WRITE, IMG_PICK, "simlod_pick_write")             \
+    X(K_NEAREST_LOCATE, IMG_NEAREST, "simlod_nearest_locate") X(K_NEAREST_SCAN, IMG_NEAREST, "simlod_nearest_scan") \
+    X(K_NEAREST_SCATTER, IMG_NEAREST, "simlod_nearest_scatter") X(K_NEAREST_SEARCH, IMG_NEAREST, "simlod_nearest_search")
 #define X(k, image, name) k,
 enum Kernel { KERNEL_LIST(X) NUM_KERNELS };
 #undef X
@@ -199,9 +203,11 @@ struct SimlodContext {
     CUevent evStaged[MAX_STAGING_SLOTS] = {}, evStagingFree[MAX_STAGING_SLOTS] = {};
     CUdeviceptr exportScratch = 0;     // octree export and region query: see scratchFor()
     uint64_t exportScratchBytes = 0;
-    void* hExportCtl = nullptr;        // pinned copy of ExportCtl / QueryCtl (CTL_HOST_BYTES)
+    void* hExportCtl = nullptr;        // pinned copy of ExportCtl / QueryCtl / NearestCtl (CTL_HOST_BYTES)
     CUdeviceptr pickScratch = 0;       // pick: key frame | index frame | hit counter | pixel list
     uint64_t pickScratchBytes = 0;
+    CUdeviceptr nearestScratch = 0;    // k nearest: per query home | slot | bucket, per home count | offset | run start, NearestCtl
+    uint64_t nearestScratchBytes = 0;
     CUdeviceptr fileWindow = 0;        // octree files: FILE_WINDOW_BYTES of samples staged on the device
     CUdeviceptr fileTables = 0;        // octree load: records | plan | error word, sized for nodes[]
     uint64_t fileTablesBytes = 0;
@@ -618,6 +624,7 @@ void simlod_destroy(SimlodContext* ctx) {
         if (ctx->exportScratch) D(cuMemFree)(ctx->exportScratch);
         if (ctx->hExportCtl) D(cuMemFreeHost)(ctx->hExportCtl);
         if (ctx->pickScratch) D(cuMemFree)(ctx->pickScratch);
+        if (ctx->nearestScratch) D(cuMemFree)(ctx->nearestScratch);
         if (ctx->fileWindow) D(cuMemFree)(ctx->fileWindow);
         if (ctx->fileTables) D(cuMemFree)(ctx->fileTables);
         delete ctx->loaderPool;          // joins the loader threads
@@ -1427,7 +1434,7 @@ int simlod_flush_l2(SimlodContext* ctx) {
 namespace {
 constexpr uint64_t align16(uint64_t v) { return (v + 15) & ~15ull; }
 constexpr size_t CTL_HOST_BYTES = 128;      // the pinned copy of the control word
-static_assert(sizeof(ExportCtl) <= CTL_HOST_BYTES && sizeof(QueryCtl) <= CTL_HOST_BYTES, "pinned control word");
+static_assert(sizeof(ExportCtl) <= CTL_HOST_BYTES && sizeof(QueryCtl) <= CTL_HOST_BYTES && sizeof(NearestCtl) <= CTL_HOST_BYTES, "pinned control word");
 
 // The context's export / query scratch, sized by its buffers: one record, node index and first item per node of nodes[],
 // and one chunk item per chunk the heap can hold. The view adds per node a drawn byte, and per record a mark byte, an
@@ -1683,6 +1690,68 @@ int simlod_pick(SimlodContext* ctx, const uint32_t* pixels, uint64_t num_pixels,
     info->num_hits = hits; info->num_samples = p.c.numSamples; info->num_nodes = p.c.numNodes; info->num_pixels = n;
     info->plan_ms = p.ms; info->key_ms = keyMs; info->index_ms = indexMs; info->write_ms = writeMs;
     if (kernel_ms) *kernel_ms = p.ms + keyMs + indexMs + writeMs;
+    return SIMLOD_OK;
+}
+
+// ---- k nearest samples (DESIGN.md §9.10); kernels in nearest.cu, the plan is the export's -------------------------------
+int simlod_query_nearest(SimlodContext* ctx, uint64_t queries, uint64_t num_queries, uint32_t k, int32_t depth, float max_radius,
+                         uint64_t dst_index, uint64_t dst_dist2, uint64_t dst_samples, SimlodNearestInfo* info, float* kernel_ms) {
+    int rc = setCurrent(ctx); if (rc) return rc;
+    if (!info) return fail(SIMLOD_ERR_INVALID, "null info");
+    if (k < 1 || k > SIMLOD_NEAREST_MAX_K) return fail(SIMLOD_ERR_INVALID, "k = %u, 1 to %d are supported", k, (int)SIMLOD_NEAREST_MAX_K);
+    if (num_queries == 0 || num_queries > SIMLOD_NEAREST_MAX_QUERIES)
+        return fail(SIMLOD_ERR_INVALID, "%llu queries, 1 to %u are supported", (unsigned long long)num_queries, (unsigned)SIMLOD_NEAREST_MAX_QUERIES);
+    if (depth > SIMLOD_MAX_DEPTH) return fail(SIMLOD_ERR_INVALID, "nearest depth %d exceeds the octree's maximum depth %d", depth, (int)SIMLOD_MAX_DEPTH);
+    if (std::isnan(max_radius) || max_radius < 0.0f) return fail(SIMLOD_ERR_INVALID, "max_radius must be >= 0 or +inf");
+    if (!queries || queries % 16) return fail(SIMLOD_ERR_INVALID, "the query array must be a 16-byte aligned device address");
+    if (dst_index % 8 || dst_dist2 % 4 || dst_samples % 16)
+        return fail(SIMLOD_ERR_INVALID, "nearest destinations must be 8-byte (indices), 4-byte (distances) and 16-byte (samples) aligned");
+    const uint32_t n = (uint32_t)num_queries;
+    // stage 1: the export's plan and chunk items, into its scratch, and the one host round trip for its control word
+    ExportPlanned p;
+    rc = exportPlan(ctx, depth < 0 ? -1 : depth, nullptr, &p);
+    if (kernel_ms) *kernel_ms = p.ms;
+    if (rc) return rc;
+    const uint32_t records = p.c.numNodes, homes = records + 1;
+    uint64_t at = 0;
+    auto take = [&](uint64_t bytes) { const uint64_t off = at; at += align16(bytes); return off; };
+    const uint64_t oHome = take(4ull * n), oSlot = take(4ull * n), oBucket = take(4ull * n);
+    const uint64_t oCount = take(4ull * homes), oOffset = take(4ull * homes), oRun = take(4ull * (homes + 1)), oCtl = take(sizeof(NearestCtl));
+    rc = growDevice(&ctx->nearestScratch, &ctx->nearestScratchBytes, at); if (rc) return rc;
+    const CUdeviceptr base = ctx->nearestScratch;
+    NearestArgs a{};
+    a.rec = devPtr(p.s.rec); a.recItem = devPtr(p.s.recItem); a.items = devPtr(p.s.items); a.queries = devPtr(queries);
+    a.home = devPtr(base + oHome); a.slot = devPtr(base + oSlot); a.bucket = devPtr(base + oBucket);
+    a.count = devPtr(base + oCount); a.offset = devPtr(base + oOffset); a.runStart = devPtr(base + oRun); a.ctl = devPtr(base + oCtl);
+    a.dstIndex = devPtr(dst_index); a.dstDist2 = devPtr(dst_dist2); a.dstSamples = devPtr(dst_samples);
+    a.numQueries = n; a.numRecords = records; a.k = k; a.depth = depth < 0 ? -1 : depth; a.maxRadius = max_radius;
+    for (int ax = 0; ax < 3; ax++) { a.boxMin[ax] = ctx->uniforms.boxMin[ax]; a.boxMax[ax] = ctx->uniforms.boxMax[ax]; }
+    // stage 2: locate and bucket the queries; stage 3: the search, which writes the destinations unless the scan found
+    // the record tree inconsistent
+    const unsigned blocks = (unsigned)std::min<uint64_t>((n + 255) / 256, (uint64_t)ctx->numSMs * 8);
+    const unsigned runs = (unsigned)((n + NEAREST_RUN - 1) / NEAREST_RUN + std::min<uint64_t>(n, homes));   // >= the runs the scan counts
+    CU(D(cuEventRecord)(ctx->evStart, ctx->streamMain));
+    CU(D(cuMemsetD32Async)(base + oCount, 0, homes, ctx->streamMain));
+    CU(D(cuMemsetD8Async)(base + oCtl, 0, sizeof(NearestCtl), ctx->streamMain));
+    rc = launch(ctx, ctx->fn[K_NEAREST_LOCATE], blocks, 256, ctx->streamMain, a); if (rc) return rc;
+    rc = launch(ctx, ctx->fn[K_NEAREST_SCAN], 1, 1024, ctx->streamMain, a); if (rc) return rc;
+    rc = launch(ctx, ctx->fn[K_NEAREST_SCATTER], blocks, 256, ctx->streamMain, a); if (rc) return rc;
+    CU(D(cuEventRecord)(ctx->evEnd, ctx->streamMain));
+    rc = launch(ctx, ctx->fn[K_NEAREST_SEARCH], runs, NEAREST_RUN * 32, ctx->streamMain, a); if (rc) return rc;
+    CU(D(cuEventRecord)(ctx->evTotalEnd, ctx->streamMain));
+    CU(D(cuMemcpyDtoHAsync)(ctx->hExportCtl, base + oCtl, sizeof(NearestCtl), ctx->streamMain));
+    CU(D(cuStreamSynchronize)(ctx->streamMain));
+    NearestCtl c;
+    memcpy(&c, ctx->hExportCtl, sizeof(c));
+    float bucketMs = 0.0f, searchMs = 0.0f;
+    CU(D(cuEventElapsedTime)(&bucketMs, ctx->evStart, ctx->evEnd));
+    CU(D(cuEventElapsedTime)(&searchMs, ctx->evEnd, ctx->evTotalEnd));
+    if (kernel_ms) *kernel_ms = p.ms + bucketMs + searchMs;
+    if (c.error) return failInconsistent(c.error);
+    *info = SimlodNearestInfo{};
+    info->num_samples = p.c.numSamples; info->num_found = c.numFound; info->samples_tested = c.samplesTested;
+    info->records_visited = c.recordsVisited; info->num_queries = n; info->k = k; info->invalid_queries = (uint32_t)c.invalid;
+    info->max_level = p.c.maxLevel; info->plan_ms = p.ms; info->bucket_ms = bucketMs; info->search_ms = searchMs;
     return SIMLOD_OK;
 }
 

@@ -1,6 +1,6 @@
 // kernel_args.h — the argument and control structs that host.cpp fills and the kernels read, with the codes and limits
 // both sides use. One definition for both compilers: plain C++ (no device code), included by host.cpp and by export.cu,
-// query.cu and pick.cu (through export_common.cuh), import.cu and partition.cu. The static_asserts pin every size, and the offsets
+// query.cu, pick.cu and nearest.cu (through export_common.cuh), import.cu and partition.cu. The static_asserts pin every size, and the offsets
 // that one side reads of a struct the other writes, so a layout change fails to compile instead of shifting bytes.
 #pragma once
 #include <stddef.h>
@@ -58,6 +58,40 @@ struct PickArgs {                         // the view export's plan (export scra
     uint32_t numRecords, pad;
 };
 static_assert(sizeof(PickArgs) == 64 && offsetof(PickArgs, numItems) == 48, "PickArgs");
+
+// ---- k nearest samples (nearest.cu) ----------------------------------------------------------------------------------
+
+constexpr uint32_t NEAREST_RUN = 8;       // queries per block of the search, one warp each
+
+struct NearestCtl {                       // zeroed by the host before the locate; read back after the search
+    uint32_t error;                       // EXPORT_ERR_CHILD: a record tree deeper than 20 levels or with levels out of step
+    uint32_t numRuns;                     // blocks the search needs: runs of up to NEAREST_RUN queries with one home
+    uint64_t numFound, samplesTested, recordsVisited, invalid;
+};
+static_assert(sizeof(NearestCtl) == 40 && offsetof(NearestCtl, numFound) == 8, "NearestCtl");
+
+struct NearestArgs {                      // the export's plan (export scratch), the query's scratch and its destinations
+    const SimlodExportNode* rec;          // [record] the plan's breadth-first records
+    const uint64_t* recItem;              // [record] first chunk item of the record's point list (its voxel list follows)
+    const uint64_t* items;                // [item] two words: Item {src, dst | count << 48} (export_common.cuh)
+    const float* queries;                 // [query] 16-byte records x, y, z, ignored
+    uint32_t* home;                       // [query] home record; numRecords for a query with a non-finite coordinate
+    uint32_t* slot;                       // [query] position in its home's bucket
+    uint32_t* count;                      // [home] queries per home record (numRecords + 1 homes)
+    uint32_t* offset;                     // [home] first bucket position of the home
+    uint32_t* runStart;                   // [home] first run of the home; [numRecords + 1] = the number of runs
+    uint32_t* bucket;                     // [position] query ids grouped by home
+    NearestCtl* ctl;
+    int64_t* dstIndex;                    // [query][k] or null
+    float* dstDist2;                      // [query][k] or null
+    SimlodPoint* dstSamples;              // [query][k] or null
+    uint32_t numQueries, numRecords, k;
+    int32_t depth;                        // < 0: the points of the leaves; else the export's cut at `depth`
+    float maxRadius;
+    float boxMin[3], boxMax[3];           // of the uniforms: the octree cube
+    uint32_t pad;
+};
+static_assert(sizeof(NearestArgs) == 160 && offsetof(NearestArgs, numQueries) == 112 && offsetof(NearestArgs, boxMin) == 132, "NearestArgs");
 
 // ---- octree import (import.cu) ------------------------------------------------------------------------------------
 
