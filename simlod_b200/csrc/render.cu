@@ -606,6 +606,10 @@ kernel_render(uint32_t* buffer, const Uniforms uniforms, Node* nodes, cudaSurfac
         ulonglong2* fb2 = reinterpret_cast<ulonglong2*>(framebuffer);
         for (uint32_t i = gtid; i < numPixels / 2; i += gstride) fb2[i] = make_ulonglong2(clearValue, clearValue);
         if ((numPixels & 1) && first) framebuffer[numPixels - 1] = clearValue;
+        // the word past the frame, in the pad before the HQS targets: EDL reads it as the neighbour below the last row
+        // (its index clamps to numPixels), so it is an empty pixel, not what the buffer last held. (The reference never
+        // writes it.) A pointSize >= 4 sample that wraps into it still atomicMins it below.
+        if (first) framebuffer[numPixels] = clearValue;
         if (hqs && uniforms.showPoints) {
             for (uint32_t i = gtid; i < numPixels; i += gstride) fb_depth[i] = 0x7f800000u;
             uint4* c4 = reinterpret_cast<uint4*>(fb_color);

@@ -50,8 +50,9 @@ def frame(fb, surface, visible, voxels, nodes=None):
     """A rendered frame: the depth word of every pixel, the visible counts, (optionally) the visibility flags of every
     node in canonical (level, X, Y, Z) order and, when no voxel is drawn (`voxels` == 0), the raw u64 framebuffer and
     the RGBA8 surface. Which point donates a voxel's colour is a race in the builders, so the colours of a frame that
-    draws voxels differ from build to build; every other colour (point colours, node / LOD colours, HQS sums, EDL) is
-    deterministic and compared bit for bit."""
+    draws voxels differ from build to build, and only voxel-free frames have their colours (point, node / LOD colours,
+    HQS sums, EDL) compared bit for bit here. The colours of every frame, voxel frames included, are compared with a
+    CPU restatement of HQS and EDL, and with the reference kernel on the same octree image, in test_frame_gpu.py."""
     out = {"depth": sha256(fb >> np.uint64(32)), "visible": [int(v) for v in visible]}
     if voxels == 0:
         out["framebuffer"] = sha256(fb)

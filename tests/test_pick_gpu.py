@@ -14,6 +14,7 @@ import pytest
 
 import oracle
 import pick_restatement as P
+from frame_restatement import covered
 from simlod_b200 import SimLOD, SimlodError, api, camera
 from test_export_gpu import build, buffer_digests, terrain_ragged_stream, uniform_stream
 from test_export_view_gpu import build_generated_terrain, view_cameras
@@ -42,15 +43,6 @@ def sim():
     s.close()
 
 
-def edl_covered(sim):
-    """Pixels whose colour word the EDL pass rewrites: the first floor(tiles / grid) * grid 16x16 tiles (render.cu)."""
-    grid = sim.launch_info()["render_blocks"]
-    tx, ty = sim.width // 16, sim.height // 16
-    covered_tiles = (tx * ty // grid) * grid
-    y, x = np.mgrid[0:sim.height, 0:sim.width]
-    return (x // 16 < tx) & (y // 16 < ty) & ((y // 16) * tx + x // 16 < covered_tiles)
-
-
 def check_frame(sim, label):
     """render(), then the whole-frame pick against the framebuffer. Returns (index, view export, uniforms)."""
     sim.render()
@@ -66,7 +58,7 @@ def check_frame(sim, label):
     hi = np.uint64(32)
     bad = (fb >> hi) != (want >> hi)
     if not u["useHighQualityShading"]:
-        bad |= (fb != want) & ~edl_covered(sim)
+        bad |= (fb != want) & ~covered(sim.width, sim.height, sim.launch_info()["render_blocks"])
     assert not bad.any(), "%s: %d pixels differ from the frame, first at %s" % (label, int(bad.sum()), np.argwhere(bad)[:3].tolist())
     return index, e, u
 
