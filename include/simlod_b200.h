@@ -322,6 +322,49 @@ SIMLOD_STATIC_ASSERT(offsetof(SimlodNearestInfo, num_queries) == 32 && offsetof(
 int simlod_query_nearest(SimlodContext* ctx, uint64_t queries, uint64_t num_queries, uint32_t k, int32_t depth, float max_radius,
                          uint64_t dst_index, uint64_t dst_dist2, uint64_t dst_samples, SimlodNearestInfo* info, float* kernel_ms);
 
+// Rays (DESIGN.md §9.11): for each ray, the first sample of a sample set along it within a radius of the ray, as an index
+// into the sample array simlod_export_octree(depth) returns for the same state.
+#define SIMLOD_RAY_MAX_RAYS (1u << 24)
+typedef struct SimlodRayInfo {
+    uint64_t num_samples;                           //   0  samples of the export at `depth`: the index space
+    uint64_t num_hits;                              //   8  rays with a hit
+    uint64_t samples_tested;                        //  16  sample evaluations, summed over the rays
+    uint64_t records_visited;                       //  24  records whose samples were evaluated, summed over the rays
+    uint32_t num_rays;                              //  32
+    uint32_t invalid_rays;                          //  36  rays refused one by one (an empty result each)
+    uint32_t max_level;                             //  40  deepest level in the octree
+    float    plan_ms, trace_ms;                     //  44  event time of the export's plan, and of the level check and
+                                                    //      the trace (which writes the destinations)
+    uint32_t reserved;                              //  52
+} SimlodRayInfo;
+SIMLOD_STATIC_ASSERT(sizeof(SimlodRayInfo) == 56, "RayInfo");
+SIMLOD_STATIC_ASSERT(offsetof(SimlodRayInfo, num_rays) == 32 && offsetof(SimlodRayInfo, plan_ms) == 44, "RayInfo.num_rays");
+//   rays         a device address of num_rays 32-byte records (ox, oy, oz, tmin, dx, dy, dz, tmax), float32, 16-byte
+//                aligned, 1 <= num_rays <= SIMLOD_RAY_MAX_RAYS
+//   direction    normalised by the library: len = sqrt((double(dx)*double(dx) + double(dy)*double(dy)) + double(dz)*double(dz)),
+//                u = float32(double(d) / len) per axis, every double operation rounded to nearest, nothing contracted
+//   invalid ray  an origin or direction that is not finite, a zero direction, tmin NaN, negative or infinite, tmax NaN
+//                or below tmin: an empty result, counted in info->invalid_rays (not an error)
+//   sample set   as simlod_query_nearest's: depth < 0, the eligible points of every leaf (the inserted point set);
+//                0 <= depth <= 20, the export's cut at `depth`, its points eligible ones, its voxels always
+//   per sample p float32 without contraction: w = p - o per axis; t = ((wx*ux + wy*uy) + wz*uz) + 0 (the + 0 turns -0
+//                into +0); c = w x u (cx = wy*uz - wz*uy, cy = wz*ux - wx*uz, cz = wx*uy - wy*ux);
+//                h2 = (cx*cx + cy*cy) + cz*cz. p is a hit when tmin <= t <= tmax and h2 <= radius*radius (float32);
+//                a NaN never hits
+//   result       per ray the hit with the smallest (t bits, index): dst_index[i] (int64, -1 for none), dst_t[i] (float32,
+//                +inf for none), dst_h2[i] (float32, +inf for none), dst_samples[i] (the 16-byte SimlodPoint, bit for bit
+//                export_octree(depth).samples[index], zeros for none)
+// Each destination may be 0 (not written). SIMLOD_ERR_INVALID before any launch, with nothing written, for a radius that
+// is negative or not finite, num_rays 0 or above SIMLOD_RAY_MAX_RAYS, depth > 20, a null or misaligned ray array or a
+// misaligned destination; with nothing written, for an inconsistent image (the export's conditions, and a record tree
+// whose levels do not step by one from the root to at most 20). A record whose inflated lattice box the ray's segment
+// cannot reach before its best hit is skipped unread, so the result equals an exhaustive search, and two calls on the
+// same state are byte-identical. Reads the ABI only, as the export does, and writes nothing into the context's buffers
+// or Stats. Enqueued on the launch stream; returns once complete. *kernel_ms (optional) = event time of all its kernels.
+// Scratch: the export's, and a 40-byte control word, kept until simlod_destroy.
+int simlod_query_ray(SimlodContext* ctx, uint64_t rays, uint64_t num_rays, float radius, int32_t depth, uint64_t dst_index,
+                     uint64_t dst_t, uint64_t dst_h2, uint64_t dst_samples, SimlodRayInfo* info, float* kernel_ms);
+
 // Octree files (SimlodOctreeFileHeader, DESIGN.md §9.7): a built octree saved and loaded back, so that it can be rendered,
 // exported or continued with new batches in another context, process or session.
 // simlod_read_octree_header: the header of an octree file, checked against itself and the file size. No context, no GPU.

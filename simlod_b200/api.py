@@ -170,6 +170,17 @@ class SimlodNearestInfo(C.Structure):
                 ("reserved", C.c_uint32)]
 
 
+RAY_MAX_RAYS = 1 << 24
+
+
+class SimlodRayInfo(C.Structure):
+    """SimlodRayInfo: the export's sample count (the index space), rays with a hit, how much of the octree the trace had
+    to look at, and the event time of each stage."""
+    _fields_ = [("num_samples", C.c_uint64), ("num_hits", C.c_uint64), ("samples_tested", C.c_uint64),
+                ("records_visited", C.c_uint64), ("num_rays", C.c_uint32), ("invalid_rays", C.c_uint32),
+                ("max_level", C.c_uint32), ("plan_ms", C.c_float), ("trace_ms", C.c_float), ("reserved", C.c_uint32)]
+
+
 class Region:
     """Constructors of the regions SimLOD.query_region takes. Numbers are rounded to float32, the type the predicates are
     evaluated in; a malformed region (non-finite number, min > max, negative radius) is refused by the query."""
@@ -214,7 +225,7 @@ assert C.sizeof(ExportInfo) == 32 and EXPORT_NODE_DTYPE.itemsize == 64
 assert C.sizeof(LasHeader) == 128
 assert C.sizeof(OctreeFileHeader) == 128
 assert C.sizeof(SimlodRegion) == 304 and C.sizeof(SimlodQueryInfo) == 40
-assert C.sizeof(SimlodPickInfo) == 40 and C.sizeof(SimlodNearestInfo) == 64
+assert C.sizeof(SimlodPickInfo) == 40 and C.sizeof(SimlodNearestInfo) == 64 and C.sizeof(SimlodRayInfo) == 56
 
 # every symbol include/simlod_b200.h declares
 EXPORTS = [
@@ -228,7 +239,7 @@ EXPORTS = [
     "simlod_export_framebuffer", "simlod_peer_signal", "simlod_composite_framebuffers", "simlod_generate", "simlod_reset_with_grid", "simlod_insert_simlod_file_ex", "simlod_get_numa_node",
     "simlod_export_octree", "simlod_export_view", "simlod_read_las_header", "simlod_insert_files",
     "simlod_read_octree_header", "simlod_save_octree", "simlod_load_octree", "simlod_query_region",
-    "simlod_pick", "simlod_query_nearest",
+    "simlod_pick", "simlod_query_nearest", "simlod_query_ray",
 ]
 
 _lib = None
@@ -295,6 +306,7 @@ def load_library():
         "simlod_pick": [vp, C.POINTER(C.c_uint32), u64, u64, u64, C.POINTER(SimlodPickInfo), C.POINTER(C.c_float)],
         "simlod_query_nearest": [vp, u64, u64, u32, C.c_int32, C.c_float, u64, u64, u64, C.POINTER(SimlodNearestInfo),
                                  C.POINTER(C.c_float)],
+        "simlod_query_ray": [vp, u64, u64, C.c_float, C.c_int32, u64, u64, u64, u64, C.POINTER(SimlodRayInfo), C.POINTER(C.c_float)],
     }
     for name, argtypes in sig.items():
         fn = getattr(lib, name)
@@ -819,6 +831,90 @@ class SimLOD:
         info, _ = self.query_nearest_into(qptr, n, k, depth, max_radius, index.data_ptr() if n else 0,
                                           dist2.data_ptr() if n else 0, found.data_ptr() if samples and n else 0)
         return (index, dist2, found, info) if samples else (index, dist2, info)
+
+    def query_ray_into(self, rays_ptr, n, radius, depth, dst_index, dst_t, dst_h2, dst_samples):
+        """simlod_query_ray on caller-owned device memory: n 32-byte ray records (ox, oy, oz, tmin, dx, dy, dz, tmax) at
+        rays_ptr, destinations [n] int64 / float32 / float32 / 16-byte samples, each 0 for not written (depth None or < 0:
+        the inserted points). Returns (SimlodRayInfo, kernel ms)."""
+        info, ms = SimlodRayInfo(), C.c_float(0)
+        d = -1 if depth is None else int(depth)
+        self._check(self._lib.simlod_query_ray(self._ctx, int(rays_ptr), int(n), float(radius), d, int(dst_index), int(dst_t),
+                                               int(dst_h2), int(dst_samples), C.byref(info), C.byref(ms)))
+        return info, ms.value
+
+    def query_ray(self, origins, directions, radius, tmin=0.0, tmax=None, depth=None, device="cuda", samples=False):
+        """The first stored sample along each ray (simlod_query_ray), exact: among the samples within `radius` of the ray
+        o + t u (u the direction normalised by the library) with tmin <= t <= tmax, the one with the least t, ties by
+        index. With depth=None among the inserted points (those on the cube's max face excepted, as query_region), with
+        an integer depth among the samples of export_octree(depth). `origins`, `directions`: (N, 3) arrays, numpy or CUDA
+        tensors; `tmin`, `tmax`: scalars or (N,) arrays (tmax None: +inf). A ray with a non-finite or zero direction, a
+        non-finite origin or a bad [tmin, tmax] gets an empty result and counts in info.invalid_rays. Returns
+        (index, t, h2, info) or, with samples=True, (index, t, h2, samples, info): (N,) int64 indices into
+        export_octree(depth).samples, -1 for no hit; (N,) float32 t, +inf for no hit; (N,) float32 squared distances
+        from the ray, +inf for no hit; (N, 4) float32 samples in the export's layout, zeros for no hit. device="cuda":
+        torch tensors in device memory; device="cpu": numpy arrays (the samples as POINT_DTYPE)."""
+        on_device = not isinstance(origins, np.ndarray) and hasattr(origins, "data_ptr")
+        if on_device:
+            import torch
+            o = origins.detach()
+            d = directions.detach() if hasattr(directions, "data_ptr") else torch.as_tensor(np.asarray(directions), device=o.device)
+            if not o.is_cuda or o.ndim != 2 or o.shape[1] != 3 or tuple(d.shape) != tuple(o.shape):
+                raise ValueError("origins and directions must be (N, 3) CUDA tensors or numpy arrays of one shape")
+            n = o.shape[0]
+            r = torch.empty((n, 8), dtype=torch.float32, device=o.device)
+            r[:, 0:3] = o.to(torch.float32)
+            r[:, 4:7] = d.to(device=o.device, dtype=torch.float32)
+            for col, v, default in ((3, tmin, 0.0), (7, tmax, float("inf"))):
+                v = default if v is None else v
+                r[:, col] = v.to(device=o.device, dtype=torch.float32) if hasattr(v, "data_ptr") else \
+                    torch.as_tensor(np.broadcast_to(np.asarray(v, dtype=np.float32), (n,)).copy(), device=o.device)
+            torch.cuda.current_stream(o.device).synchronize()  # the rays may still be being computed on torch's stream
+            return self._ray(r.data_ptr(), n, radius, depth, device, samples)
+        o, d = np.asarray(origins), np.asarray(directions)
+        if o.ndim != 2 or o.shape[1] != 3 or d.shape != o.shape:
+            raise ValueError("origins and directions must be (N, 3) CUDA tensors or numpy arrays of one shape")
+        n = o.shape[0]
+        r = np.empty((n, 8), dtype=np.float32)
+        r[:, 0:3], r[:, 4:7] = o, d
+        r[:, 3] = np.broadcast_to(np.asarray(0.0 if tmin is None else tmin, dtype=np.float32), (n,))
+        r[:, 7] = np.broadcast_to(np.asarray(np.inf if tmax is None else tmax, dtype=np.float32), (n,))
+        dr = self.device_alloc(max(r.nbytes, 32))
+        try:
+            self.memcpy_htod(dr, r)
+            return self._ray(dr, n, radius, depth, device, samples)
+        finally:
+            self.device_free(dr)
+
+    def _ray(self, rptr, n, radius, depth, device, samples):
+        if device == "cpu":
+            m = max(n, 1)
+            di, dt, dh = self.device_alloc(m * 8), self.device_alloc(m * 4), self.device_alloc(m * 4)
+            ds = self.device_alloc(m * 16) if samples else 0
+            try:
+                info, _ = self.query_ray_into(rptr, n, radius, depth, di, dt, dh, ds)
+                index = self.memcpy_dtoh(di, n * 8).view(np.int64)
+                t = self.memcpy_dtoh(dt, n * 4).view(np.float32)
+                h2 = self.memcpy_dtoh(dh, n * 4).view(np.float32)
+                found = self.memcpy_dtoh(ds, n * 16).view(POINT_DTYPE) if samples else None
+            finally:
+                for p in (di, dt, dh, ds):
+                    if p:
+                        self.device_free(p)
+            return (index, t, h2, found, info) if samples else (index, t, h2, info)
+        import torch
+        dev = torch.device(device)
+        if dev.type != "cuda":
+            raise ValueError("device must be 'cpu' or a CUDA device, not %r" % device)
+        if dev.index is None:
+            dev = torch.device("cuda", self.device)
+        index = torch.empty(n, dtype=torch.int64, device=dev)
+        t = torch.empty(n, dtype=torch.float32, device=dev)
+        h2 = torch.empty(n, dtype=torch.float32, device=dev)
+        found = torch.empty((n, 4), dtype=torch.float32, device=dev) if samples else None
+        torch.cuda.current_stream(dev).synchronize()       # the caching allocator may hand out memory torch still uses
+        info, _ = self.query_ray_into(rptr, n, radius, depth, index.data_ptr() if n else 0, t.data_ptr() if n else 0,
+                                      h2.data_ptr() if n else 0, found.data_ptr() if samples and n else 0)
+        return (index, t, h2, found, info) if samples else (index, t, h2, info)
 
     def host_alloc(self, nbytes):
         p = C.c_void_p()

@@ -69,3 +69,22 @@ def autofocus(box_size, width, height, yaw_offset=0.0):
 
 MORRO_BIRD = dict(yaw=-0.207, pitch=-0.797, radius=3866.886, target=(2398.747, 2167.120, -394.165))
 MORRO_CLOSE = dict(yaw=-11.270, pitch=-0.225, radius=93.982, target=(2750.218, 974.775, 76.230))
+
+
+def pixel_rays(view, proj, width, height, pixels=None):
+    """World-space rays through the centres of pixels of a width x height frame: (origins, directions), (N, 3) float64,
+    the origin the camera's position, the direction from the near to the far plane through (x + 0.5, y + 0.5), with
+    NDC y = 2 (y + 0.5) / height - 1. pixels: an (N, 2) array of (x, y), or None for every pixel, row by row. For
+    SimLOD.query_ray."""
+    if pixels is None:
+        ys, xs = np.mgrid[0:height, 0:width]
+        pixels = np.stack([xs.ravel(), ys.ravel()], axis=1)
+    p = np.asarray(pixels, dtype=np.float64).reshape(-1, 2)
+    ndc = np.stack([2.0 * (p[:, 0] + 0.5) / width - 1.0, 2.0 * (p[:, 1] + 0.5) / height - 1.0], axis=1)
+    inv = np.linalg.inv(np.asarray(proj, dtype=np.float64) @ np.asarray(view, dtype=np.float64))
+    ends = []
+    for z in (-1.0, 1.0):
+        h = np.concatenate([ndc, np.full((len(p), 1), z), np.ones((len(p), 1))], axis=1) @ inv.T
+        ends.append(h[:, :3] / h[:, 3:4])
+    origin = np.linalg.inv(np.asarray(view, dtype=np.float64))[:3, 3]
+    return np.tile(origin, (len(p), 1)), ends[1] - ends[0]

@@ -1,5 +1,6 @@
-// export_common.cuh — what the export (export.cu) and the region query (query.cu) share: the chunk item and the
-// block-wide scan of their one-block plan kernels. The control word and its inconsistency codes are in kernel_args.h.
+// export_common.cuh — what the export (export.cu) and the queries built on its plan (query.cu, pick.cu, nearest.cu, ray.cu)
+// share: the chunk item, the block-wide scan of the one-block plan kernels and the record tree's level check. The control
+// word and its inconsistency codes are in kernel_args.h.
 #pragma once
 #include <stdint.h>
 #include "../../include/simlod_abi.h"
@@ -21,6 +22,19 @@ __device__ __forceinline__ uint32_t itemRecord(uint64_t k, const uint64_t* __res
         if (recItem[mid] <= k) lo = mid; else hi = mid;
     }
     return lo;
+}
+
+// Whether record r breaks the level rule the searches of nearest.cu and ray.cu rely on: the root at level 0, every
+// child one level below its parent, no inner record at level 20. With it a depth-first walk that pushes at most 8 children
+// per pop never holds more than 7 * 20 + 1 records.
+__device__ __forceinline__ bool levelOutOfStep(const SimlodExportNode* rec, uint32_t r) {
+    const SimlodExportNode& n = rec[r];
+    bool bad = r == 0 && n.level != 0;
+    if (n.first_child >= 0) {
+        if (n.level >= SIMLOD_MAX_DEPTH) bad = true;
+        for (uint32_t k = 0; k < 8; k++) bad = bad || rec[(uint32_t)n.first_child + k].level != n.level + 1;
+    }
+    return bad;
 }
 
 // Block-wide exclusive scan (PLAN_THREADS threads) of 64-bit values; returns the prefix, *total the sum. One instance per

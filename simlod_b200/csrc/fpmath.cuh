@@ -75,6 +75,12 @@ __device__ __forceinline__ double dmul(double a, double b) {
 __device__ __forceinline__ double dadd(double a, double b) {
     double r; asm("add.rn.f64 %0, %1, %2;" : "=d"(r) : "d"(a), "d"(b)); return r;
 }
+__device__ __forceinline__ double ddiv(double a, double b) {   // correctly rounded: numpy's float64 a / b
+    double r; asm("div.rn.f64 %0, %1, %2;" : "=d"(r) : "d"(a), "d"(b)); return r;
+}
+__device__ __forceinline__ double dsqrt(double a) {            // correctly rounded: numpy's float64 sqrt
+    double r; asm("sqrt.rn.f64 %0, %1;" : "=d"(r) : "d"(a)); return r;
+}
 __device__ __forceinline__ int32_t d2i(double a) {       // F2I.F64.TRUNC
     int32_t r; asm("cvt.rzi.s32.f64 %0, %1;" : "=r"(r) : "d"(a)); return r;
 }

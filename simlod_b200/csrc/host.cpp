@@ -50,6 +50,7 @@ extern const unsigned char simlod_cubin_import[];
 extern const unsigned char simlod_cubin_query[];
 extern const unsigned char simlod_cubin_pick[];
 extern const unsigned char simlod_cubin_nearest[];
+extern const unsigned char simlod_cubin_ray[];
 }
 
 namespace {
@@ -115,10 +116,10 @@ struct Program {
 
 // The embedded images of the kernels that are launched outside the three swappable programs, and those kernels: one
 // row each, {enum value, image, kernel name}. createResources loads every image and looks up every kernel.
-enum Image { IMG_UTIL, IMG_LAS, IMG_GEN, IMG_PARTITION, IMG_EXPORT, IMG_QUERY, IMG_IMPORT, IMG_PICK, IMG_NEAREST, NUM_IMAGES };
+enum Image { IMG_UTIL, IMG_LAS, IMG_GEN, IMG_PARTITION, IMG_EXPORT, IMG_QUERY, IMG_IMPORT, IMG_PICK, IMG_NEAREST, IMG_RAY, NUM_IMAGES };
 const unsigned char* const IMAGES[NUM_IMAGES] = {simlod_cubin_util, simlod_cubin_las, simlod_cubin_gen, simlod_cubin_partition,
                                                  simlod_cubin_export, simlod_cubin_query, simlod_cubin_import, simlod_cubin_pick,
-                                                 simlod_cubin_nearest};
+                                                 simlod_cubin_nearest, simlod_cubin_ray};
 #define KERNEL_LIST(X)                                                                                    \
     X(K_RCP, IMG_UTIL, "simlod_util_rcp") X(K_FILL, IMG_UTIL, "simlod_util_fill")                         \
     X(K_LAS, IMG_LAS, "simlod_las_decode")                                                                \
@@ -139,7 +140,8 @@ const unsigned char* const IMAGES[NUM_IMAGES] = {simlod_cubin_util, simlod_cubin
     X(K_PICK_CLEAR, IMG_PICK, "simlod_pick_clear") X(K_PICK_KEY, IMG_PICK, "simlod_pick_key")             \
     X(K_PICK_INDEX, IMG_PICK, "simlod_pick_index") X(K_PICK_WRITE, IMG_PICK, "simlod_pick_write")             \
     X(K_NEAREST_LOCATE, IMG_NEAREST, "simlod_nearest_locate") X(K_NEAREST_SCAN, IMG_NEAREST, "simlod_nearest_scan") \
-    X(K_NEAREST_SCATTER, IMG_NEAREST, "simlod_nearest_scatter") X(K_NEAREST_SEARCH, IMG_NEAREST, "simlod_nearest_search")
+    X(K_NEAREST_SCATTER, IMG_NEAREST, "simlod_nearest_scatter") X(K_NEAREST_SEARCH, IMG_NEAREST, "simlod_nearest_search") \
+    X(K_RAY_CHECK, IMG_RAY, "simlod_ray_check") X(K_RAY_TRACE, IMG_RAY, "simlod_ray_trace")
 #define X(k, image, name) k,
 enum Kernel { KERNEL_LIST(X) NUM_KERNELS };
 #undef X
@@ -203,11 +205,13 @@ struct SimlodContext {
     CUevent evStaged[MAX_STAGING_SLOTS] = {}, evStagingFree[MAX_STAGING_SLOTS] = {};
     CUdeviceptr exportScratch = 0;     // octree export and region query: see scratchFor()
     uint64_t exportScratchBytes = 0;
-    void* hExportCtl = nullptr;        // pinned copy of ExportCtl / QueryCtl / NearestCtl (CTL_HOST_BYTES)
+    void* hExportCtl = nullptr;        // pinned copy of ExportCtl / QueryCtl / NearestCtl / RayCtl (CTL_HOST_BYTES)
     CUdeviceptr pickScratch = 0;       // pick: key frame | index frame | hit counter | pixel list
     uint64_t pickScratchBytes = 0;
     CUdeviceptr nearestScratch = 0;    // k nearest: per query home | slot | bucket, per home count | offset | run start, NearestCtl
     uint64_t nearestScratchBytes = 0;
+    CUdeviceptr rayCtl = 0;            // rays: RayCtl
+    uint64_t rayCtlBytes = 0;
     CUdeviceptr fileWindow = 0;        // octree files: FILE_WINDOW_BYTES of samples staged on the device
     CUdeviceptr fileTables = 0;        // octree load: records | plan | error word, sized for nodes[]
     uint64_t fileTablesBytes = 0;
@@ -625,6 +629,7 @@ void simlod_destroy(SimlodContext* ctx) {
         if (ctx->hExportCtl) D(cuMemFreeHost)(ctx->hExportCtl);
         if (ctx->pickScratch) D(cuMemFree)(ctx->pickScratch);
         if (ctx->nearestScratch) D(cuMemFree)(ctx->nearestScratch);
+        if (ctx->rayCtl) D(cuMemFree)(ctx->rayCtl);
         if (ctx->fileWindow) D(cuMemFree)(ctx->fileWindow);
         if (ctx->fileTables) D(cuMemFree)(ctx->fileTables);
         delete ctx->loaderPool;          // joins the loader threads
@@ -1434,7 +1439,8 @@ int simlod_flush_l2(SimlodContext* ctx) {
 namespace {
 constexpr uint64_t align16(uint64_t v) { return (v + 15) & ~15ull; }
 constexpr size_t CTL_HOST_BYTES = 128;      // the pinned copy of the control word
-static_assert(sizeof(ExportCtl) <= CTL_HOST_BYTES && sizeof(QueryCtl) <= CTL_HOST_BYTES && sizeof(NearestCtl) <= CTL_HOST_BYTES, "pinned control word");
+static_assert(sizeof(ExportCtl) <= CTL_HOST_BYTES && sizeof(QueryCtl) <= CTL_HOST_BYTES && sizeof(NearestCtl) <= CTL_HOST_BYTES &&
+              sizeof(RayCtl) <= CTL_HOST_BYTES, "pinned control word");
 
 // The context's export / query scratch, sized by its buffers: one record, node index and first item per node of nodes[],
 // and one chunk item per chunk the heap can hold. The view adds per node a drawn byte, and per record a mark byte, an
@@ -1752,6 +1758,53 @@ int simlod_query_nearest(SimlodContext* ctx, uint64_t queries, uint64_t num_quer
     info->num_samples = p.c.numSamples; info->num_found = c.numFound; info->samples_tested = c.samplesTested;
     info->records_visited = c.recordsVisited; info->num_queries = n; info->k = k; info->invalid_queries = (uint32_t)c.invalid;
     info->max_level = p.c.maxLevel; info->plan_ms = p.ms; info->bucket_ms = bucketMs; info->search_ms = searchMs;
+    return SIMLOD_OK;
+}
+
+// ---- rays (DESIGN.md §9.11); kernels in ray.cu, the plan is the export's ------------------------------------------------
+int simlod_query_ray(SimlodContext* ctx, uint64_t rays, uint64_t num_rays, float radius, int32_t depth, uint64_t dst_index,
+                     uint64_t dst_t, uint64_t dst_h2, uint64_t dst_samples, SimlodRayInfo* info, float* kernel_ms) {
+    int rc = setCurrent(ctx); if (rc) return rc;
+    if (!info) return fail(SIMLOD_ERR_INVALID, "null info");
+    if (!std::isfinite(radius) || radius < 0.0f) return fail(SIMLOD_ERR_INVALID, "radius must be finite and >= 0");
+    if (num_rays == 0 || num_rays > SIMLOD_RAY_MAX_RAYS)
+        return fail(SIMLOD_ERR_INVALID, "%llu rays, 1 to %u are supported", (unsigned long long)num_rays, (unsigned)SIMLOD_RAY_MAX_RAYS);
+    if (depth > SIMLOD_MAX_DEPTH) return fail(SIMLOD_ERR_INVALID, "ray depth %d exceeds the octree's maximum depth %d", depth, (int)SIMLOD_MAX_DEPTH);
+    if (!rays || rays % 16) return fail(SIMLOD_ERR_INVALID, "the ray array must be a 16-byte aligned device address");
+    if (dst_index % 8 || dst_t % 4 || dst_h2 % 4 || dst_samples % 16)
+        return fail(SIMLOD_ERR_INVALID, "ray destinations must be 8-byte (indices), 4-byte (t, h2) and 16-byte (samples) aligned");
+    const uint32_t n = (uint32_t)num_rays;
+    // stage 1: the export's plan and chunk items, into its scratch, and the one host round trip for its control word
+    ExportPlanned p;
+    rc = exportPlan(ctx, depth < 0 ? -1 : depth, nullptr, &p);
+    if (kernel_ms) *kernel_ms = p.ms;
+    if (rc) return rc;
+    rc = growDevice(&ctx->rayCtl, &ctx->rayCtlBytes, sizeof(RayCtl)); if (rc) return rc;
+    RayArgs a{};
+    a.rec = devPtr(p.s.rec); a.recItem = devPtr(p.s.recItem); a.items = devPtr(p.s.items); a.rays = devPtr(rays);
+    a.ctl = devPtr(ctx->rayCtl);
+    a.dstIndex = devPtr(dst_index); a.dstT = devPtr(dst_t); a.dstH2 = devPtr(dst_h2); a.dstSamples = devPtr(dst_samples);
+    a.numRays = n; a.numRecords = p.c.numNodes; a.depth = depth < 0 ? -1 : depth; a.radius = radius;
+    for (int ax = 0; ax < 3; ax++) { a.boxMin[ax] = ctx->uniforms.boxMin[ax]; a.boxMax[ax] = ctx->uniforms.boxMax[ax]; }
+    // stage 2: the level check, then the trace, which writes the destinations unless the check found the record tree
+    // inconsistent
+    CU(D(cuEventRecord)(ctx->evStart, ctx->streamMain));
+    CU(D(cuMemsetD8Async)(ctx->rayCtl, 0, sizeof(RayCtl), ctx->streamMain));
+    rc = launch(ctx, ctx->fn[K_RAY_CHECK], 1, 1024, ctx->streamMain, a); if (rc) return rc;
+    rc = launch(ctx, ctx->fn[K_RAY_TRACE], (n + RAY_WARPS - 1) / RAY_WARPS, RAY_WARPS * 32, ctx->streamMain, a); if (rc) return rc;
+    CU(D(cuEventRecord)(ctx->evEnd, ctx->streamMain));
+    CU(D(cuMemcpyDtoHAsync)(ctx->hExportCtl, ctx->rayCtl, sizeof(RayCtl), ctx->streamMain));
+    CU(D(cuStreamSynchronize)(ctx->streamMain));
+    RayCtl c;
+    memcpy(&c, ctx->hExportCtl, sizeof(c));
+    float traceMs = 0.0f;
+    CU(D(cuEventElapsedTime)(&traceMs, ctx->evStart, ctx->evEnd));
+    if (kernel_ms) *kernel_ms = p.ms + traceMs;
+    if (c.error) return failInconsistent(c.error);
+    *info = SimlodRayInfo{};
+    info->num_samples = p.c.numSamples; info->num_hits = c.numHits; info->samples_tested = c.samplesTested;
+    info->records_visited = c.recordsVisited; info->num_rays = n; info->invalid_rays = (uint32_t)c.invalid;
+    info->max_level = p.c.maxLevel; info->plan_ms = p.ms; info->trace_ms = traceMs;
     return SIMLOD_OK;
 }
 

@@ -1,7 +1,8 @@
 // kernel_args.h — the argument and control structs that host.cpp fills and the kernels read, with the codes and limits
 // both sides use. One definition for both compilers: plain C++ (no device code), included by host.cpp and by export.cu,
-// query.cu, pick.cu and nearest.cu (through export_common.cuh), import.cu and partition.cu. The static_asserts pin every size, and the offsets
-// that one side reads of a struct the other writes, so a layout change fails to compile instead of shifting bytes.
+// query.cu, pick.cu, nearest.cu and ray.cu (through export_common.cuh), import.cu and partition.cu. The static_asserts pin
+// every size, and the offsets that one side reads of a struct the other writes, so a layout change fails to compile instead
+// of shifting bytes.
 #pragma once
 #include <stddef.h>
 #include <stdint.h>
@@ -92,6 +93,34 @@ struct NearestArgs {                      // the export's plan (export scratch),
     uint32_t pad;
 };
 static_assert(sizeof(NearestArgs) == 160 && offsetof(NearestArgs, numQueries) == 112 && offsetof(NearestArgs, boxMin) == 132, "NearestArgs");
+
+// ---- rays (ray.cu) ---------------------------------------------------------------------------------------------------
+
+constexpr uint32_t RAY_WARPS = 8;         // rays per block of the trace, one warp each
+
+struct RayCtl {                           // zeroed by the host before the check; read back after the trace
+    uint32_t error;                       // EXPORT_ERR_CHILD: a record tree deeper than 20 levels or with levels out of step
+    uint32_t pad;
+    uint64_t numHits, samplesTested, recordsVisited, invalid;
+};
+static_assert(sizeof(RayCtl) == 40 && offsetof(RayCtl, numHits) == 8, "RayCtl");
+
+struct RayArgs {                          // the export's plan (export scratch), the rays and the destinations
+    const SimlodExportNode* rec;          // [record] the plan's breadth-first records
+    const uint64_t* recItem;              // [record] first chunk item of the record's point list (its voxel list follows)
+    const uint64_t* items;                // [item] two words: Item {src, dst | count << 48} (export_common.cuh)
+    const float* rays;                    // [ray] 32-byte records ox, oy, oz, tmin, dx, dy, dz, tmax
+    RayCtl* ctl;
+    int64_t* dstIndex;                    // [ray] or null
+    float* dstT;                          // [ray] or null
+    float* dstH2;                         // [ray] or null
+    SimlodPoint* dstSamples;              // [ray] or null
+    uint32_t numRays, numRecords;
+    int32_t depth;                        // < 0: the points of the leaves; else the export's cut at `depth`
+    float radius;
+    float boxMin[3], boxMax[3];           // of the uniforms: the octree cube
+};
+static_assert(sizeof(RayArgs) == 112 && offsetof(RayArgs, numRays) == 72 && offsetof(RayArgs, boxMin) == 88, "RayArgs");
 
 // ---- octree import (import.cu) ------------------------------------------------------------------------------------
 

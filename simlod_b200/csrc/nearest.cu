@@ -155,14 +155,7 @@ simlod_nearest_scan(const NearestArgs a) {
         const uint64_t pr = blockScan<false>((c + RUN - 1) / RUN, &tr);
         if (r < homes) { a.offset[r] = (uint32_t)(queryBase + pq); a.runStart[r] = (uint32_t)(runBase + pr); }
         queryBase += tq; runBase += tr;
-        if (r < a.numRecords) {
-            const SimlodExportNode& n = a.rec[r];
-            if (r == 0 && n.level != 0) bad = true;
-            if (n.first_child >= 0) {
-                if (n.level >= SIMLOD_MAX_DEPTH) bad = true;
-                for (uint32_t k = 0; k < 8; k++) bad = bad || a.rec[(uint32_t)n.first_child + k].level != n.level + 1;
-            }
-        }
+        if (r < a.numRecords && levelOutOfStep(a.rec, r)) bad = true;
     }
     bad = __syncthreads_or(bad);
     if (threadIdx.x == 0) {
