@@ -365,6 +365,56 @@ SIMLOD_STATIC_ASSERT(offsetof(SimlodRayInfo, num_rays) == 32 && offsetof(SimlodR
 int simlod_query_ray(SimlodContext* ctx, uint64_t rays, uint64_t num_rays, float radius, int32_t depth, uint64_t dst_index,
                      uint64_t dst_t, uint64_t dst_h2, uint64_t dst_samples, SimlodRayInfo* info, float* kernel_ms);
 
+// Fixed-radius neighbourhoods (DESIGN.md §9.12): for each query position, every sample of a sample set within a radius
+// of it, in CSR form, as indices into the sample array simlod_export_octree(depth) returns for the same state.
+#define SIMLOD_RADIUS_MAX_QUERIES (1u << 24)
+typedef struct SimlodRadiusInfo {
+    uint64_t num_samples;                           //   0  samples of the export at `depth`: the index space
+    uint64_t num_found;                             //   8  neighbours summed over the queries (= offsets[num_queries])
+    uint64_t samples_tested;                        //  16  distance evaluations of the count pass, summed over the queries
+    uint64_t records_visited;                       //  24  records whose samples were evaluated, summed over the queries
+    uint32_t num_queries;                           //  32
+    uint32_t invalid_queries;                       //  36  queries with a non-finite coordinate (empty neighbourhood)
+    uint32_t max_level;                             //  40  deepest level in the octree
+    uint32_t max_found;                             //  44  the largest neighbourhood
+    float    plan_ms, bucket_ms, count_ms, write_ms;   //  48  event time of the export's plan, of the locate + bucketing,
+                                                    //      of the count pass + the offset scan, and of the write pass
+} SimlodRadiusInfo;
+SIMLOD_STATIC_ASSERT(sizeof(SimlodRadiusInfo) == 64, "RadiusInfo");
+SIMLOD_STATIC_ASSERT(offsetof(SimlodRadiusInfo, num_queries) == 32 && offsetof(SimlodRadiusInfo, plan_ms) == 48, "RadiusInfo.num_queries");
+//   sample set   as simlod_query_nearest's: depth < 0, the eligible points of every leaf (the inserted point set);
+//                0 <= depth <= 20, the export's cut at `depth`, its points eligible ones, its voxels always
+//   neighbour    sample p of query q when d2 <= radius * radius (float32), with d = p - q per coordinate and
+//                d2 = (dx*dx + dy*dy) + dz*dz in float32 without contraction (simlod_query_nearest's key). radius must
+//                be finite and >= 0; when radius * radius overflows to +inf every sample of the set is a neighbour,
+//                including those whose d2 overflowed
+//   queries      as simlod_query_nearest's: a device address of num_queries 16-byte records (x, y, z, one ignored
+//                word), 16-byte aligned, 1 <= num_queries <= SIMLOD_RADIUS_MAX_QUERIES, so the samples of an export, a
+//                region query or a pick can be passed as they are; queries may lie outside the cube. A query with a
+//                non-finite coordinate gets an empty neighbourhood and counts in info->invalid_queries
+//   result       CSR: dst_offsets (int64, num_queries + 1 entries, offsets[0] = 0); query q's neighbours are
+//                [offsets[q], offsets[q+1]) of dst_index (int64 indices into export_octree(depth).samples), dst_dist2
+//                (float32 d2) and dst_samples (optional, the 16-byte SimlodPoint, bit for bit the export's sample)
+//   order        within a query, the terminal records (records without children) in Z-order: by
+//                morton(X, Y, Z at the record's level) << 3 * (20 - level), child index bits x<<2 | y<<1 | z, root
+//                first (the record tree's depth-first pre-order with children in octant order); within a record the
+//                export's order (points, then voxels). Not ascending index: the export is breadth-first
+// dst_index, dst_dist2 and dst_samples all 0: a size query, which fills *info and, when dst_offsets is not 0, the offsets.
+// Otherwise `capacity` is the number of neighbour slots of each non-null destination: below info->num_found the call is
+// refused with SIMLOD_ERR_INVALID, nothing written into any destination (offsets included) and *info filled. Each of
+// dst_index, dst_dist2, dst_samples and dst_offsets may be 0 (not written). SIMLOD_ERR_INVALID before any launch, with
+// nothing written, for a radius that is NaN, negative or infinite, num_queries 0 or above SIMLOD_RADIUS_MAX_QUERIES,
+// depth > 20, a null or misaligned query array or a misaligned destination (8 / 8 / 4 / 16 bytes); with nothing written,
+// for an inconsistent image (the export's conditions, and a record tree whose levels do not step by one from the root
+// to at most 20). A record whose lattice box cannot hold a neighbour is skipped unread, so the result equals an
+// exhaustive search, and two calls on the same state are byte-identical. Reads the ABI only, as the export does, and
+// writes nothing into the context's buffers or Stats. Enqueued on the launch stream; returns once complete.
+// *kernel_ms (optional) = event time of all its kernels. Scratch: the export's, simlod_query_nearest's, and 16 bytes per
+// query, kept until simlod_destroy.
+int simlod_query_radius(SimlodContext* ctx, uint64_t queries, uint64_t num_queries, float radius, int32_t depth,
+                        uint64_t dst_offsets, uint64_t dst_index, uint64_t dst_dist2, uint64_t dst_samples,
+                        uint64_t capacity, SimlodRadiusInfo* info, float* kernel_ms);
+
 // Octree files (SimlodOctreeFileHeader, DESIGN.md §9.7): a built octree saved and loaded back, so that it can be rendered,
 // exported or continued with new batches in another context, process or session.
 // simlod_read_octree_header: the header of an octree file, checked against itself and the file size. No context, no GPU.

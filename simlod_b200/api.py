@@ -15,6 +15,7 @@ observed through Stats):
 
 There is no fallback: if libsimlod_b200.so is missing or no H100 is present, construction raises.
 """
+import contextlib
 import ctypes as C
 import os
 
@@ -181,6 +182,18 @@ class SimlodRayInfo(C.Structure):
                 ("max_level", C.c_uint32), ("plan_ms", C.c_float), ("trace_ms", C.c_float), ("reserved", C.c_uint32)]
 
 
+RADIUS_MAX_QUERIES = 1 << 24
+
+
+class SimlodRadiusInfo(C.Structure):
+    """SimlodRadiusInfo: the export's sample count (the index space), the neighbours found (offsets[-1]), how much of the
+    octree the count pass had to look at, the largest neighbourhood, and the event time of each stage."""
+    _fields_ = [("num_samples", C.c_uint64), ("num_found", C.c_uint64), ("samples_tested", C.c_uint64),
+                ("records_visited", C.c_uint64), ("num_queries", C.c_uint32), ("invalid_queries", C.c_uint32),
+                ("max_level", C.c_uint32), ("max_found", C.c_uint32), ("plan_ms", C.c_float), ("bucket_ms", C.c_float),
+                ("count_ms", C.c_float), ("write_ms", C.c_float)]
+
+
 class Region:
     """Constructors of the regions SimLOD.query_region takes. Numbers are rounded to float32, the type the predicates are
     evaluated in; a malformed region (non-finite number, min > max, negative radius) is refused by the query."""
@@ -226,6 +239,7 @@ assert C.sizeof(LasHeader) == 128
 assert C.sizeof(OctreeFileHeader) == 128
 assert C.sizeof(SimlodRegion) == 304 and C.sizeof(SimlodQueryInfo) == 40
 assert C.sizeof(SimlodPickInfo) == 40 and C.sizeof(SimlodNearestInfo) == 64 and C.sizeof(SimlodRayInfo) == 56
+assert C.sizeof(SimlodRadiusInfo) == 64
 
 # every symbol include/simlod_b200.h declares
 EXPORTS = [
@@ -239,7 +253,7 @@ EXPORTS = [
     "simlod_export_framebuffer", "simlod_peer_signal", "simlod_composite_framebuffers", "simlod_generate", "simlod_reset_with_grid", "simlod_insert_simlod_file_ex", "simlod_get_numa_node",
     "simlod_export_octree", "simlod_export_view", "simlod_read_las_header", "simlod_insert_files",
     "simlod_read_octree_header", "simlod_save_octree", "simlod_load_octree", "simlod_query_region",
-    "simlod_pick", "simlod_query_nearest", "simlod_query_ray",
+    "simlod_pick", "simlod_query_nearest", "simlod_query_ray", "simlod_query_radius",
 ]
 
 _lib = None
@@ -307,6 +321,8 @@ def load_library():
         "simlod_query_nearest": [vp, u64, u64, u32, C.c_int32, C.c_float, u64, u64, u64, C.POINTER(SimlodNearestInfo),
                                  C.POINTER(C.c_float)],
         "simlod_query_ray": [vp, u64, u64, C.c_float, C.c_int32, u64, u64, u64, u64, C.POINTER(SimlodRayInfo), C.POINTER(C.c_float)],
+        "simlod_query_radius": [vp, u64, u64, C.c_float, C.c_int32, u64, u64, u64, u64, u64, C.POINTER(SimlodRadiusInfo),
+                                C.POINTER(C.c_float)],
     }
     for name, argtypes in sig.items():
         fn = getattr(lib, name)
@@ -778,6 +794,15 @@ class SimLOD:
         (N, k) int64 indices into export_octree(depth).samples, -1 in an empty slot; (N, k) float32 squared distances,
         +inf in an empty slot; (N, k, 4) float32 samples in the export's layout, zeros in an empty slot. device="cuda":
         torch tensors in device memory; device="cpu": numpy arrays (the samples as POINT_DTYPE)."""
+        with self._device_queries(queries) as (qptr, n):
+            return self._nearest(qptr, n, k, depth, max_radius, device, samples)
+
+    @contextlib.contextmanager
+    def _device_queries(self, queries):
+        """The query records query_nearest and query_radius take, as 16-byte records (x, y, z, ignored word) at a device
+        address: yields (address, count). `queries`: an (N, 3) or (N, 4) array (the 4th column is ignored), numpy or a
+        CUDA tensor, or POINT_DTYPE samples. A contiguous float32 (N, 4) CUDA tensor at a 16-byte aligned address is
+        passed as it is; anything else is copied, into memory freed when the block ends."""
         if isinstance(queries, np.ndarray) and queries.dtype == POINT_DTYPE:
             queries = queries.view(np.float32).reshape(-1, 4)
         if not isinstance(queries, np.ndarray) and hasattr(queries, "data_ptr"):
@@ -790,7 +815,8 @@ class SimLOD:
                 q4[:, :3] = q[:, :3]
                 q = q4
             torch.cuda.current_stream(q.device).synchronize()  # the queries may still be being computed on torch's stream
-            return self._nearest(q.data_ptr(), q.shape[0], k, depth, max_radius, device, samples, keep=q)
+            yield q.data_ptr(), q.shape[0]                      # q stays alive until the block ends
+            return
         a = np.asarray(queries)
         if a.ndim != 2 or a.shape[1] not in (3, 4):
             raise ValueError("queries must be an (N, 3) or (N, 4) CUDA tensor or numpy array")
@@ -799,11 +825,11 @@ class SimLOD:
         dq = self.device_alloc(max(q.nbytes, 16))
         try:
             self.memcpy_htod(dq, q)
-            return self._nearest(dq, q.shape[0], k, depth, max_radius, device, samples)
+            yield dq, q.shape[0]
         finally:
             self.device_free(dq)
 
-    def _nearest(self, qptr, n, k, depth, max_radius, device, samples, keep=None):
+    def _nearest(self, qptr, n, k, depth, max_radius, device, samples):
         if device == "cpu":
             m = max(n * k, 1)
             di, dd = self.device_alloc(m * 8), self.device_alloc(m * 4)
@@ -831,6 +857,64 @@ class SimLOD:
         info, _ = self.query_nearest_into(qptr, n, k, depth, max_radius, index.data_ptr() if n else 0,
                                           dist2.data_ptr() if n else 0, found.data_ptr() if samples and n else 0)
         return (index, dist2, found, info) if samples else (index, dist2, info)
+
+    def query_radius_into(self, queries_ptr, n, radius, depth, dst_offsets, dst_index, dst_dist2, dst_samples, capacity):
+        """simlod_query_radius on caller-owned device memory: n 16-byte query records at queries_ptr; dst_offsets int64
+        [n + 1]; dst_index / dst_dist2 / dst_samples int64 / float32 / 16-byte samples with `capacity` neighbour slots
+        each, 0 for not written (all three 0: size query, which fills the offsets when dst_offsets is not 0; depth None or
+        < 0: the inserted points). Returns (SimlodRadiusInfo, kernel ms)."""
+        info, ms = SimlodRadiusInfo(), C.c_float(0)
+        d = -1 if depth is None else int(depth)
+        self._check(self._lib.simlod_query_radius(self._ctx, int(queries_ptr), int(n), float(radius), d, int(dst_offsets),
+                                                  int(dst_index), int(dst_dist2), int(dst_samples), int(capacity),
+                                                  C.byref(info), C.byref(ms)))
+        return info, ms.value
+
+    def query_radius(self, queries, radius, depth=None, device="cuda", samples=False):
+        """Every sample within `radius` of each query position (simlod_query_radius), exact: with depth=None among the
+        inserted points (those on the cube's max face excepted, as query_region), with an integer depth among the
+        samples of export_octree(depth). A sample is a neighbour when its squared distance in float32, the k-nearest
+        query's key, is <= radius * radius. `queries` as query_nearest takes them. The result is in CSR form: query q's
+        neighbours are [offsets[q], offsets[q + 1]) of index (int64 indices into export_octree(depth).samples), dist2
+        (float32) and, with samples=True, samples ((M, 4) float32 in the export's layout). Within a query the records
+        come in Z-order and each record's samples in the export's order (not sorted by distance or index). A query with
+        a non-finite coordinate has no neighbours and counts in info.invalid_queries. One size query, then the full
+        call. Returns (offsets, index, dist2, info) or, with samples=True, (offsets, index, dist2, samples, info).
+        device="cuda": torch tensors in device memory; device="cpu": numpy arrays (the samples as POINT_DTYPE)."""
+        with self._device_queries(queries) as (qptr, n):
+            info, _ = self.query_radius_into(qptr, n, radius, depth, 0, 0, 0, 0, 0)
+            m = info.num_found
+            if device == "cpu":
+                do = self.device_alloc((n + 1) * 8)
+                di, dd = self.device_alloc(max(m, 1) * 8), self.device_alloc(max(m, 1) * 4)
+                ds = self.device_alloc(max(m, 1) * 16) if samples else 0
+                try:
+                    info, _ = self.query_radius_into(qptr, n, radius, depth, do, di, dd, ds, m)
+                    offsets = self.memcpy_dtoh(do, (n + 1) * 8).view(np.int64)
+                    index = self.memcpy_dtoh(di, m * 8).view(np.int64)
+                    dist2 = self.memcpy_dtoh(dd, m * 4).view(np.float32)
+                    found = self.memcpy_dtoh(ds, m * 16).view(POINT_DTYPE) if samples else None
+                finally:
+                    for p in (do, di, dd, ds):
+                        if p:
+                            self.device_free(p)
+                return (offsets, index, dist2, found, info) if samples else (offsets, index, dist2, info)
+            import torch
+            dev = torch.device(device)
+            if dev.type != "cuda":
+                raise ValueError("device must be 'cpu' or a CUDA device, not %r" % device)
+            if dev.index is None:
+                dev = torch.device("cuda", self.device)
+            offsets = torch.empty(n + 1, dtype=torch.int64, device=dev)
+            index = torch.empty(max(m, 1), dtype=torch.int64, device=dev)
+            dist2 = torch.empty(max(m, 1), dtype=torch.float32, device=dev)
+            found = torch.empty((max(m, 1), 4), dtype=torch.float32, device=dev) if samples else None
+            torch.cuda.current_stream(dev).synchronize()       # the caching allocator may hand out memory torch still uses
+            info, _ = self.query_radius_into(qptr, n, radius, depth, offsets.data_ptr(), index.data_ptr(), dist2.data_ptr(),
+                                             found.data_ptr() if samples else 0, m)
+            index, dist2 = index[:m], dist2[:m]
+            found = found[:m] if samples else None
+            return (offsets, index, dist2, found, info) if samples else (offsets, index, dist2, info)
 
     def query_ray_into(self, rays_ptr, n, radius, depth, dst_index, dst_t, dst_h2, dst_samples):
         """simlod_query_ray on caller-owned device memory: n 32-byte ray records (ox, oy, oz, tmin, dx, dy, dz, tmax) at

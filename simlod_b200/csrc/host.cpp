@@ -51,6 +51,7 @@ extern const unsigned char simlod_cubin_query[];
 extern const unsigned char simlod_cubin_pick[];
 extern const unsigned char simlod_cubin_nearest[];
 extern const unsigned char simlod_cubin_ray[];
+extern const unsigned char simlod_cubin_radius[];
 }
 
 namespace {
@@ -116,10 +117,10 @@ struct Program {
 
 // The embedded images of the kernels that are launched outside the three swappable programs, and those kernels: one
 // row each, {enum value, image, kernel name}. createResources loads every image and looks up every kernel.
-enum Image { IMG_UTIL, IMG_LAS, IMG_GEN, IMG_PARTITION, IMG_EXPORT, IMG_QUERY, IMG_IMPORT, IMG_PICK, IMG_NEAREST, IMG_RAY, NUM_IMAGES };
+enum Image { IMG_UTIL, IMG_LAS, IMG_GEN, IMG_PARTITION, IMG_EXPORT, IMG_QUERY, IMG_IMPORT, IMG_PICK, IMG_NEAREST, IMG_RAY, IMG_RADIUS, NUM_IMAGES };
 const unsigned char* const IMAGES[NUM_IMAGES] = {simlod_cubin_util, simlod_cubin_las, simlod_cubin_gen, simlod_cubin_partition,
                                                  simlod_cubin_export, simlod_cubin_query, simlod_cubin_import, simlod_cubin_pick,
-                                                 simlod_cubin_nearest, simlod_cubin_ray};
+                                                 simlod_cubin_nearest, simlod_cubin_ray, simlod_cubin_radius};
 #define KERNEL_LIST(X)                                                                                    \
     X(K_RCP, IMG_UTIL, "simlod_util_rcp") X(K_FILL, IMG_UTIL, "simlod_util_fill")                         \
     X(K_LAS, IMG_LAS, "simlod_las_decode")                                                                \
@@ -141,7 +142,9 @@ const unsigned char* const IMAGES[NUM_IMAGES] = {simlod_cubin_util, simlod_cubin
     X(K_PICK_INDEX, IMG_PICK, "simlod_pick_index") X(K_PICK_WRITE, IMG_PICK, "simlod_pick_write")             \
     X(K_NEAREST_LOCATE, IMG_NEAREST, "simlod_nearest_locate") X(K_NEAREST_SCAN, IMG_NEAREST, "simlod_nearest_scan") \
     X(K_NEAREST_SCATTER, IMG_NEAREST, "simlod_nearest_scatter") X(K_NEAREST_SEARCH, IMG_NEAREST, "simlod_nearest_search") \
-    X(K_RAY_CHECK, IMG_RAY, "simlod_ray_check") X(K_RAY_TRACE, IMG_RAY, "simlod_ray_trace")
+    X(K_RAY_CHECK, IMG_RAY, "simlod_ray_check") X(K_RAY_TRACE, IMG_RAY, "simlod_ray_trace")                 \
+    X(K_RADIUS_COUNT, IMG_RADIUS, "simlod_radius_count") X(K_RADIUS_REDUCE, IMG_RADIUS, "simlod_radius_reduce") \
+    X(K_RADIUS_SCAN, IMG_RADIUS, "simlod_radius_scan") X(K_RADIUS_WRITE, IMG_RADIUS, "simlod_radius_write")
 #define X(k, image, name) k,
 enum Kernel { KERNEL_LIST(X) NUM_KERNELS };
 #undef X
@@ -1440,7 +1443,7 @@ namespace {
 constexpr uint64_t align16(uint64_t v) { return (v + 15) & ~15ull; }
 constexpr size_t CTL_HOST_BYTES = 128;      // the pinned copy of the control word
 static_assert(sizeof(ExportCtl) <= CTL_HOST_BYTES && sizeof(QueryCtl) <= CTL_HOST_BYTES && sizeof(NearestCtl) <= CTL_HOST_BYTES &&
-              sizeof(RayCtl) <= CTL_HOST_BYTES, "pinned control word");
+              sizeof(RayCtl) <= CTL_HOST_BYTES && sizeof(NearestCtl) + sizeof(RadiusCtl) <= CTL_HOST_BYTES, "pinned control word");
 
 // The context's export / query scratch, sized by its buffers: one record, node index and first item per node of nodes[],
 // and one chunk item per chunk the heap can hold. The view adds per node a drawn byte, and per record a mark byte, an
@@ -1700,6 +1703,43 @@ int simlod_pick(SimlodContext* ctx, const uint32_t* pixels, uint64_t num_pixels,
 }
 
 // ---- k nearest samples (DESIGN.md §9.10); kernels in nearest.cu, the plan is the export's -------------------------------
+namespace {
+// The queries bucketed by home record (nearest.cu's locate, scan and scatter), in the context's nearest scratch: per query
+// home | slot | bucket, per home count | offset | run start, NearestCtl, then `extraBytes` for the caller at *extra.
+// Fills the NearestArgs of the bucketing (no destinations) and enqueues its clears and three kernels.
+int launchBuckets(SimlodContext* ctx, const ExportPlanned& p, uint64_t queries, uint32_t n, int32_t depth, uint64_t extraBytes,
+                  NearestArgs* out, CUdeviceptr* extra) {
+    const uint32_t records = p.c.numNodes, homes = records + 1;
+    uint64_t at = 0;
+    auto take = [&](uint64_t bytes) { const uint64_t off = at; at += align16(bytes); return off; };
+    const uint64_t oHome = take(4ull * n), oSlot = take(4ull * n), oBucket = take(4ull * n);
+    const uint64_t oCount = take(4ull * homes), oOffset = take(4ull * homes), oRun = take(4ull * (homes + 1)), oCtl = take(sizeof(NearestCtl));
+    const uint64_t oExtra = take(extraBytes);
+    int rc = growDevice(&ctx->nearestScratch, &ctx->nearestScratchBytes, at); if (rc) return rc;
+    const CUdeviceptr base = ctx->nearestScratch;
+    NearestArgs a{};
+    a.rec = devPtr(p.s.rec); a.recItem = devPtr(p.s.recItem); a.items = devPtr(p.s.items); a.queries = devPtr(queries);
+    a.home = devPtr(base + oHome); a.slot = devPtr(base + oSlot); a.bucket = devPtr(base + oBucket);
+    a.count = devPtr(base + oCount); a.offset = devPtr(base + oOffset); a.runStart = devPtr(base + oRun); a.ctl = devPtr(base + oCtl);
+    a.numQueries = n; a.numRecords = records; a.k = 1; a.depth = depth < 0 ? -1 : depth; a.maxRadius = INFINITY;
+    for (int ax = 0; ax < 3; ax++) { a.boxMin[ax] = ctx->uniforms.boxMin[ax]; a.boxMax[ax] = ctx->uniforms.boxMax[ax]; }
+    *out = a;
+    if (extra) *extra = base + oExtra;
+    const unsigned blocks = (unsigned)std::min<uint64_t>((n + 255) / 256, (uint64_t)ctx->numSMs * 8);
+    CU(D(cuMemsetD32Async)(base + oCount, 0, homes, ctx->streamMain));
+    CU(D(cuMemsetD8Async)(base + oCtl, 0, sizeof(NearestCtl), ctx->streamMain));
+    rc = launch(ctx, ctx->fn[K_NEAREST_LOCATE], blocks, 256, ctx->streamMain, a); if (rc) return rc;
+    rc = launch(ctx, ctx->fn[K_NEAREST_SCAN], 1, 1024, ctx->streamMain, a); if (rc) return rc;
+    return launch(ctx, ctx->fn[K_NEAREST_SCATTER], blocks, 256, ctx->streamMain, a);
+}
+
+// The grid of a search over the buckets: the upper bound ceil(n / NEAREST_RUN) + min(n, homes) of the runs the scan
+// counts; the blocks beyond return
+unsigned searchRuns(uint32_t n, uint32_t records) {
+    return (unsigned)((n + NEAREST_RUN - 1) / NEAREST_RUN + std::min<uint64_t>(n, (uint64_t)records + 1));
+}
+}  // namespace
+
 int simlod_query_nearest(SimlodContext* ctx, uint64_t queries, uint64_t num_queries, uint32_t k, int32_t depth, float max_radius,
                          uint64_t dst_index, uint64_t dst_dist2, uint64_t dst_samples, SimlodNearestInfo* info, float* kernel_ms) {
     int rc = setCurrent(ctx); if (rc) return rc;
@@ -1718,34 +1758,17 @@ int simlod_query_nearest(SimlodContext* ctx, uint64_t queries, uint64_t num_quer
     rc = exportPlan(ctx, depth < 0 ? -1 : depth, nullptr, &p);
     if (kernel_ms) *kernel_ms = p.ms;
     if (rc) return rc;
-    const uint32_t records = p.c.numNodes, homes = records + 1;
-    uint64_t at = 0;
-    auto take = [&](uint64_t bytes) { const uint64_t off = at; at += align16(bytes); return off; };
-    const uint64_t oHome = take(4ull * n), oSlot = take(4ull * n), oBucket = take(4ull * n);
-    const uint64_t oCount = take(4ull * homes), oOffset = take(4ull * homes), oRun = take(4ull * (homes + 1)), oCtl = take(sizeof(NearestCtl));
-    rc = growDevice(&ctx->nearestScratch, &ctx->nearestScratchBytes, at); if (rc) return rc;
-    const CUdeviceptr base = ctx->nearestScratch;
-    NearestArgs a{};
-    a.rec = devPtr(p.s.rec); a.recItem = devPtr(p.s.recItem); a.items = devPtr(p.s.items); a.queries = devPtr(queries);
-    a.home = devPtr(base + oHome); a.slot = devPtr(base + oSlot); a.bucket = devPtr(base + oBucket);
-    a.count = devPtr(base + oCount); a.offset = devPtr(base + oOffset); a.runStart = devPtr(base + oRun); a.ctl = devPtr(base + oCtl);
-    a.dstIndex = devPtr(dst_index); a.dstDist2 = devPtr(dst_dist2); a.dstSamples = devPtr(dst_samples);
-    a.numQueries = n; a.numRecords = records; a.k = k; a.depth = depth < 0 ? -1 : depth; a.maxRadius = max_radius;
-    for (int ax = 0; ax < 3; ax++) { a.boxMin[ax] = ctx->uniforms.boxMin[ax]; a.boxMax[ax] = ctx->uniforms.boxMax[ax]; }
     // stage 2: locate and bucket the queries; stage 3: the search, which writes the destinations unless the scan found
     // the record tree inconsistent
-    const unsigned blocks = (unsigned)std::min<uint64_t>((n + 255) / 256, (uint64_t)ctx->numSMs * 8);
-    const unsigned runs = (unsigned)((n + NEAREST_RUN - 1) / NEAREST_RUN + std::min<uint64_t>(n, homes));   // >= the runs the scan counts
     CU(D(cuEventRecord)(ctx->evStart, ctx->streamMain));
-    CU(D(cuMemsetD32Async)(base + oCount, 0, homes, ctx->streamMain));
-    CU(D(cuMemsetD8Async)(base + oCtl, 0, sizeof(NearestCtl), ctx->streamMain));
-    rc = launch(ctx, ctx->fn[K_NEAREST_LOCATE], blocks, 256, ctx->streamMain, a); if (rc) return rc;
-    rc = launch(ctx, ctx->fn[K_NEAREST_SCAN], 1, 1024, ctx->streamMain, a); if (rc) return rc;
-    rc = launch(ctx, ctx->fn[K_NEAREST_SCATTER], blocks, 256, ctx->streamMain, a); if (rc) return rc;
+    NearestArgs a{};
+    rc = launchBuckets(ctx, p, queries, n, depth, 0, &a, nullptr); if (rc) return rc;
+    a.dstIndex = devPtr(dst_index); a.dstDist2 = devPtr(dst_dist2); a.dstSamples = devPtr(dst_samples);
+    a.k = k; a.maxRadius = max_radius;
     CU(D(cuEventRecord)(ctx->evEnd, ctx->streamMain));
-    rc = launch(ctx, ctx->fn[K_NEAREST_SEARCH], runs, NEAREST_RUN * 32, ctx->streamMain, a); if (rc) return rc;
+    rc = launch(ctx, ctx->fn[K_NEAREST_SEARCH], searchRuns(n, p.c.numNodes), NEAREST_RUN * 32, ctx->streamMain, a); if (rc) return rc;
     CU(D(cuEventRecord)(ctx->evTotalEnd, ctx->streamMain));
-    CU(D(cuMemcpyDtoHAsync)(ctx->hExportCtl, base + oCtl, sizeof(NearestCtl), ctx->streamMain));
+    CU(D(cuMemcpyDtoHAsync)(ctx->hExportCtl, (CUdeviceptr)(uintptr_t)a.ctl, sizeof(NearestCtl), ctx->streamMain));
     CU(D(cuStreamSynchronize)(ctx->streamMain));
     NearestCtl c;
     memcpy(&c, ctx->hExportCtl, sizeof(c));
@@ -1758,6 +1781,91 @@ int simlod_query_nearest(SimlodContext* ctx, uint64_t queries, uint64_t num_quer
     info->num_samples = p.c.numSamples; info->num_found = c.numFound; info->samples_tested = c.samplesTested;
     info->records_visited = c.recordsVisited; info->num_queries = n; info->k = k; info->invalid_queries = (uint32_t)c.invalid;
     info->max_level = p.c.maxLevel; info->plan_ms = p.ms; info->bucket_ms = bucketMs; info->search_ms = searchMs;
+    return SIMLOD_OK;
+}
+
+// ---- fixed-radius neighbourhoods (DESIGN.md §9.12); kernels in radius.cu after nearest.cu's bucketing -------------------
+int simlod_query_radius(SimlodContext* ctx, uint64_t queries, uint64_t num_queries, float radius, int32_t depth,
+                        uint64_t dst_offsets, uint64_t dst_index, uint64_t dst_dist2, uint64_t dst_samples,
+                        uint64_t capacity, SimlodRadiusInfo* info, float* kernel_ms) {
+    int rc = setCurrent(ctx); if (rc) return rc;
+    if (!info) return fail(SIMLOD_ERR_INVALID, "null info");
+    if (!std::isfinite(radius) || radius < 0.0f) return fail(SIMLOD_ERR_INVALID, "radius must be finite and >= 0");
+    if (num_queries == 0 || num_queries > SIMLOD_RADIUS_MAX_QUERIES)
+        return fail(SIMLOD_ERR_INVALID, "%llu queries, 1 to %u are supported", (unsigned long long)num_queries, (unsigned)SIMLOD_RADIUS_MAX_QUERIES);
+    if (depth > SIMLOD_MAX_DEPTH) return fail(SIMLOD_ERR_INVALID, "radius depth %d exceeds the octree's maximum depth %d", depth, (int)SIMLOD_MAX_DEPTH);
+    if (!queries || queries % 16) return fail(SIMLOD_ERR_INVALID, "the query array must be a 16-byte aligned device address");
+    if (dst_offsets % 8 || dst_index % 8 || dst_dist2 % 4 || dst_samples % 16)
+        return fail(SIMLOD_ERR_INVALID, "radius destinations must be 8-byte (offsets, indices), 4-byte (distances) and 16-byte (samples) aligned");
+    const uint32_t n = (uint32_t)num_queries;
+    const bool sizeQuery = !dst_index && !dst_dist2 && !dst_samples;
+    // stage 1: the export's plan and chunk items, into its scratch, and the one host round trip for its control word
+    ExportPlanned p;
+    rc = exportPlan(ctx, depth < 0 ? -1 : depth, nullptr, &p);
+    if (kernel_ms) *kernel_ms = p.ms;
+    if (rc) return rc;
+    // stage 2: locate and bucket the queries (nearest.cu); stage 3: count, reduce and scan, then one host round trip
+    const uint32_t tiles = (n + RADIUS_SCAN_TILE - 1) / RADIUS_SCAN_TILE;
+    uint64_t at = 0;
+    auto take = [&](uint64_t bytes) { const uint64_t off = at; at += align16(bytes); return off; };
+    const uint64_t oCtl = take(sizeof(RadiusCtl)), oTotal = take(4ull * n), oBefore = take(4ull * n), oTile = take(8ull * tiles);
+    const uint64_t oOffsets = take(8ull * (n + 1));
+    CU(D(cuEventRecord)(ctx->evStart, ctx->streamMain));
+    NearestArgs na{};
+    CUdeviceptr base = 0;
+    rc = launchBuckets(ctx, p, queries, n, depth, at, &na, &base); if (rc) return rc;
+    RadiusArgs a{};
+    a.rec = na.rec; a.recItem = na.recItem; a.items = na.items; a.queries = na.queries;
+    a.count = na.count; a.offset = na.offset; a.runStart = na.runStart; a.bucket = na.bucket; a.nearestCtl = na.ctl;
+    a.ctl = devPtr(base + oCtl); a.total = devPtr(base + oTotal); a.before = devPtr(base + oBefore); a.tileSum = devPtr(base + oTile);
+    a.offsets = devPtr(base + oOffsets);
+    a.dstIndex = devPtr(dst_index); a.dstDist2 = devPtr(dst_dist2); a.dstSamples = devPtr(dst_samples);
+    a.numQueries = n; a.numRecords = p.c.numNodes; a.depth = na.depth; a.radius = radius;
+    for (int ax = 0; ax < 3; ax++) { a.boxMin[ax] = na.boxMin[ax]; a.boxMax[ax] = na.boxMax[ax]; }
+    CU(D(cuMemsetD8Async)(base + oCtl, 0, sizeof(RadiusCtl), ctx->streamMain));
+    CU(D(cuEventRecord)(ctx->evEnd, ctx->streamMain));
+    const unsigned runs = searchRuns(n, p.c.numNodes);
+    rc = launch(ctx, ctx->fn[K_RADIUS_COUNT], runs, NEAREST_RUN * 32, ctx->streamMain, a); if (rc) return rc;
+    rc = launch(ctx, ctx->fn[K_RADIUS_REDUCE], tiles, 1024, ctx->streamMain, a); if (rc) return rc;
+    rc = launch(ctx, ctx->fn[K_RADIUS_SCAN], tiles, 1024, ctx->streamMain, a); if (rc) return rc;
+    CU(D(cuEventRecord)(ctx->evTotalEnd, ctx->streamMain));
+    uint8_t* const hc = (uint8_t*)ctx->hExportCtl;
+    CU(D(cuMemcpyDtoHAsync)(hc, (CUdeviceptr)(uintptr_t)na.ctl, sizeof(NearestCtl), ctx->streamMain));
+    CU(D(cuMemcpyDtoHAsync)(hc + sizeof(NearestCtl), base + oCtl, sizeof(RadiusCtl), ctx->streamMain));
+    CU(D(cuStreamSynchronize)(ctx->streamMain));
+    NearestCtl nc;
+    RadiusCtl c;
+    memcpy(&nc, hc, sizeof(nc));
+    memcpy(&c, hc + sizeof(NearestCtl), sizeof(c));
+    float bucketMs = 0.0f, countMs = 0.0f;
+    CU(D(cuEventElapsedTime)(&bucketMs, ctx->evStart, ctx->evEnd));
+    CU(D(cuEventElapsedTime)(&countMs, ctx->evEnd, ctx->evTotalEnd));
+    if (kernel_ms) *kernel_ms = p.ms + bucketMs + countMs;
+    if (nc.error) return failInconsistent(nc.error);
+    *info = SimlodRadiusInfo{};
+    info->num_samples = p.c.numSamples; info->num_found = c.numFound; info->samples_tested = c.samplesTested;
+    info->records_visited = c.recordsVisited; info->num_queries = n; info->invalid_queries = (uint32_t)c.invalid;
+    info->max_level = p.c.maxLevel; info->max_found = c.maxFound;
+    info->plan_ms = p.ms; info->bucket_ms = bucketMs; info->count_ms = countMs;
+    if (sizeQuery) {                                            // size query: the offsets at most
+        if (dst_offsets) {
+            CU(D(cuMemcpyDtoDAsync)((CUdeviceptr)dst_offsets, base + oOffsets, 8ull * (n + 1), ctx->streamMain));
+            CU(D(cuStreamSynchronize)(ctx->streamMain));
+        }
+        return SIMLOD_OK;
+    }
+    if (capacity < c.numFound)
+        return fail(SIMLOD_ERR_INVALID, "radius destinations hold %llu neighbours, the query finds %llu", (unsigned long long)capacity, (unsigned long long)c.numFound);
+    // stage 4: the offsets, and the write pass, which places every neighbour
+    CU(D(cuEventRecord)(ctx->evTotalStart, ctx->streamMain));
+    if (dst_offsets) CU(D(cuMemcpyDtoDAsync)((CUdeviceptr)dst_offsets, base + oOffsets, 8ull * (n + 1), ctx->streamMain));
+    rc = launch(ctx, ctx->fn[K_RADIUS_WRITE], runs, NEAREST_RUN * 32, ctx->streamMain, a); if (rc) return rc;
+    CU(D(cuEventRecord)(ctx->evTotalEnd, ctx->streamMain));
+    CU(D(cuEventSynchronize)(ctx->evTotalEnd));
+    float writeMs = 0.0f;
+    CU(D(cuEventElapsedTime)(&writeMs, ctx->evTotalStart, ctx->evTotalEnd));
+    info->write_ms = writeMs;
+    if (kernel_ms) *kernel_ms = p.ms + bucketMs + countMs + writeMs;
     return SIMLOD_OK;
 }
 

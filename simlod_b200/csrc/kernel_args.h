@@ -1,6 +1,6 @@
 // kernel_args.h — the argument and control structs that host.cpp fills and the kernels read, with the codes and limits
 // both sides use. One definition for both compilers: plain C++ (no device code), included by host.cpp and by export.cu,
-// query.cu, pick.cu, nearest.cu and ray.cu (through export_common.cuh), import.cu and partition.cu. The static_asserts pin
+// query.cu, pick.cu, nearest.cu, radius.cu and ray.cu (through export_common.cuh), import.cu and partition.cu. The static_asserts pin
 // every size, and the offsets that one side reads of a struct the other writes, so a layout change fails to compile instead
 // of shifting bytes.
 #pragma once
@@ -93,6 +93,43 @@ struct NearestArgs {                      // the export's plan (export scratch),
     uint32_t pad;
 };
 static_assert(sizeof(NearestArgs) == 160 && offsetof(NearestArgs, numQueries) == 112 && offsetof(NearestArgs, boxMin) == 132, "NearestArgs");
+
+// ---- fixed-radius neighbourhoods (radius.cu, after nearest.cu's locate, scan and scatter) ----------------------------
+
+constexpr uint32_t RADIUS_SCAN_ITEMS = 8;                       // counts per thread of the offset scan
+constexpr uint32_t RADIUS_SCAN_TILE = 1024 * RADIUS_SCAN_ITEMS; // counts per block of the offset scan
+
+struct RadiusCtl {                        // zeroed by the host before the locate; read back after the scan
+    uint64_t numFound, samplesTested, recordsVisited, invalid;   // summed by the count pass
+    uint32_t maxFound, pad;
+};
+static_assert(sizeof(RadiusCtl) == 40 && offsetof(RadiusCtl, maxFound) == 32, "RadiusCtl");
+
+struct RadiusArgs {                       // the export's plan (export scratch), nearest.cu's buckets, the pass scratch and
+                                          // the destinations
+    const SimlodExportNode* rec;          // [record] the plan's breadth-first records
+    const uint64_t* recItem;              // [record] first chunk item of the record's point list (its voxel list follows)
+    const uint64_t* items;                // [item] two words: Item {src, dst | count << 48} (export_common.cuh)
+    const float* queries;                 // [query] 16-byte records x, y, z, ignored
+    const uint32_t* count;                // [home] queries per home record (numRecords + 1 homes), from the locate
+    const uint32_t* offset;               // [home] first bucket position of the home
+    const uint32_t* runStart;             // [home] first run of the home; [numRecords + 1] = the number of runs
+    const uint32_t* bucket;               // [position] query ids grouped by home
+    const NearestCtl* nearestCtl;         // the scan's error and number of runs
+    RadiusCtl* ctl;
+    uint32_t* total;                      // [query] neighbours
+    uint32_t* before;                     // [query] neighbours in terminal records before the home in Z-order
+    uint64_t* tileSum;                    // [scan tile] sum of its totals
+    int64_t* offsets;                     // [query + 1] exclusive prefix of the totals
+    int64_t* dstIndex;                    // [neighbour] or null
+    float* dstDist2;                      // [neighbour] or null
+    SimlodPoint* dstSamples;              // [neighbour] or null
+    uint32_t numQueries, numRecords;
+    int32_t depth;                        // < 0: the points of the leaves; else the export's cut at `depth`
+    float radius;
+    float boxMin[3], boxMax[3];           // of the uniforms: the octree cube
+};
+static_assert(sizeof(RadiusArgs) == 176 && offsetof(RadiusArgs, numQueries) == 136 && offsetof(RadiusArgs, boxMin) == 152, "RadiusArgs");
 
 // ---- rays (ray.cu) ---------------------------------------------------------------------------------------------------
 

@@ -22,6 +22,7 @@
 #include "lodcut.cuh"
 #include "export_common.cuh"
 #include "region.cuh"
+#include "search_common.cuh"
 
 constexpr uint32_t RUN = NEAREST_RUN;
 constexpr uint32_t TILE = 1024;                                 // home candidates staged in shared memory per round
@@ -36,38 +37,6 @@ static_assert(RUN * 32 <= 1024 && SIMLOD_NEAREST_MAX_K <= 32, "one warp per quer
 // bits order as the float does.
 __device__ __forceinline__ bool keyLess(uint32_t d, uint64_t i, uint32_t kd, uint64_t ki) {
     return d < kd || (d == kd && i < ki);
-}
-
-__device__ __forceinline__ float dist2(float x, float y, float z, float qx, float qy, float qz) {
-    const float dx = fpx::sub(x, qx), dy = fpx::sub(y, qy), dz = fpx::sub(z, qz);
-    return fpx::add(fpx::add(fpx::mul(dx, dx), fpx::mul(dy, dy)), fpx::mul(dz, dz));
-}
-
-// The candidates of a terminal record, and its chunk items: points first, then (depth >= 0) voxels
-__device__ __forceinline__ uint32_t candidateCount(const SimlodExportNode& r, int32_t depth) {
-    return depth < 0 ? r.num_points : r.num_points + r.num_voxels;
-}
-
-// Lower bound of the exact squared distance from q to any eligible sample of a record, by §9.8's argument (query.cu
-// regionMisses): the lattice box inflated by `margin`, evaluated in double. fmax drops a NaN, so the bound is never NaN.
-__device__ __forceinline__ double lowerBound(const SimlodExportNode& r, const QueryCube& c, double margin, float qx, float qy, float qz) {
-    const NodeBox b = nodeBox(r.level, r.X, r.Y, r.Z, c.size, c.minx, c.miny, c.minz);
-    const float q[3] = {qx, qy, qz};
-    double d2 = 0.0;
-#pragma unroll
-    for (int a = 0; a < 3; a++) {
-        const double lo = (double)b.mn[a] - margin, hi = (double)b.mx[a] + margin, v = (double)q[a];
-        const double d = fmax(fmax(lo - v, v - hi), 0.0);
-        d2 += d * d;
-    }
-    return d2;
-}
-
-// A record is skipped when its bound exceeds this: the float key of a sample beyond it is above min(k-th key, r*r),
-// since the float sum's relative error is below 2^-21 (twice that allowed) and 1e-44 covers products that underflow.
-// Strictly above: such a sample cannot tie the k-th key either. +inf (fewer than k found, no radius) skips nothing.
-__device__ __forceinline__ double skipAbove(uint32_t kd, float rr) {
-    return (double)fminf(__uint_as_float(kd), rr) * (1.0 + 0x1p-20) + 1e-44;
 }
 
 // The warp's top-k: lane j < k holds slot j (d, index, source address), ascending. Every lane offers at most one
@@ -268,9 +237,7 @@ simlod_nearest_search(const NearestArgs a) {
 
     // the rest of the tree, one warp per query, depth first from the root with the nearest child on top
     if (active && searched) {
-        const double cubeMax = fmax(fmax(fmax(fabs((double)c.minx), fabs((double)c.miny)), fabs((double)c.minz)),
-                                    fmax(fmax(fabs((double)c.minx + c.size), fabs((double)c.miny + c.size)), fabs((double)c.minz + c.size)));
-        const double margin = (double)c.size * 0x1p-19 + cubeMax * 0x1p-21;
+        const double margin = searchMargin(c);
         uint32_t* const sRec = stRec[warp];
         double* const sBound = stBound[warp];
         if (lane == 0) { sRec[0] = 0; sBound[0] = 0.0; }
