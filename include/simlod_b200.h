@@ -440,6 +440,59 @@ int simlod_save_octree(SimlodContext* ctx, const char* path, SimlodExportInfo* i
 //                       voxels in one cell, a failed read): the context is left reset to an empty octree with the file's box.
 int simlod_load_octree(SimlodContext* ctx, const char* path, int loader_threads, SimlodExportInfo* info, float* kernel_ms);
 
+// LAS files written on the GPU (DESIGN.md §9.13): samples quantised and encoded into LAS 1.2 point-format-2 records on
+// the device, so that other tools can read what the library holds.
+typedef struct SimlodLasWriteParams {
+    double scale[3];                                //   0  > 0 and finite
+    double offset[3];                               //  24  the file's offset, finite
+    double translation[3];                          //  48  added to every sample: world = sample + translation, finite
+    uint32_t writer_threads;                        //  72  1..64 threads write the file
+    uint32_t reserved;                              //  76
+} SimlodLasWriteParams;
+SIMLOD_STATIC_ASSERT(sizeof(SimlodLasWriteParams) == 80, "LasWriteParams");
+SIMLOD_STATIC_ASSERT(offsetof(SimlodLasWriteParams, translation) == 48 && offsetof(SimlodLasWriteParams, writer_threads) == 72, "LasWriteParams.translation");
+typedef struct SimlodLasWriteInfo {
+    uint64_t num_points;                            //   0  records written
+    uint64_t file_size;                             //   8  227 + 26 * num_points
+    uint64_t first_invalid;                         //  16  source index of the first invalid sample, UINT64_MAX for none
+    double   min[3];                                //  24  the header's bounds: double(q_min) * scale + offset
+    double   max[3];                                //  48      and double(q_max) * scale + offset (0 when empty)
+    float    plan_ms;                               //  72  event time of the export's plan + collect (octree source)
+    float    encode_ms;                             //  76  event time of the gathers and encodes
+    float    copy_ms;                               //  80  event time of the device-to-host copies of the records
+    float    write_ms;                              //  84  wall time from the first window to the renamed file
+    uint32_t num_windows;                           //  88  windows of at most 8 Mi samples
+    uint32_t reserved;                              //  92
+} SimlodLasWriteInfo;
+SIMLOD_STATIC_ASSERT(sizeof(SimlodLasWriteInfo) == 96, "LasWriteInfo");
+SIMLOD_STATIC_ASSERT(offsetof(SimlodLasWriteInfo, min) == 24 && offsetof(SimlodLasWriteInfo, plan_ms) == 72 && offsetof(SimlodLasWriteInfo, num_windows) == 88, "LasWriteInfo.min");
+//   source       samples != 0: num_samples 16-byte samples (x, y, z, colour bits) at that 16-byte aligned device address,
+//                depth < 0 (the layout of export_*, query_region and the queries' samples). samples == 0: the octree's
+//                samples as the last completed launch left it, depth < 0 the inserted points (the export's cut at 20,
+//                the points on the cube's max face included), 0 <= depth <= 20 the export's cut at depth; num_samples
+//                is then ignored. Record i of the file is sample i of the source (export_octree(depth).samples, with
+//                depth 20 for depth < 0).
+//   quantised    per axis in IEEE double, nothing contracted: q = rint(((double(p) + translation) - offset) / scale),
+//                half to even. A sample with a non-finite coordinate or a q outside int32 is invalid.
+//   file         LAS 1.2, 227-byte header, no VLRs, point format 2 (26 bytes: int32 X, Y, Z = q, intensity 0, flags
+//                0x09, classification, scan angle, user data and point source 0, R, G, B = 257 * colour bits 0-7,
+//                8-15, 16-23); generating software "simlod_b200", creation day and year 0; legacy point count n and
+//                points by return [n, 0, 0, 0, 0]; scale and offset as given; min / max as in SimlodLasWriteInfo.
+// SIMLOD_ERR_INVALID before any launch, with no file created, for a null path, params or info, a scale that is not
+// finite or <= 0, a non-finite offset or translation, a misaligned samples address, samples != 0 with depth >= 0,
+// depth > 20, more than 2^32 - 1 samples of the caller's, writer_threads outside 1..64, or a path whose directory
+// cannot be written. SIMLOD_ERR_INVALID during the write for an invalid sample (info->first_invalid names the first one
+// in source order), more than 2^32 - 1 samples of the octree's, an inconsistent image or an I/O error. The file is
+// written as path + ".tmp" and renamed once complete: a failed call leaves no file and any existing file at `path` as
+// it was. Writes nothing into the context's buffers or Stats. *kernel_ms (optional) = event time of all its kernels.
+// Staging: the file streamer's page-locked pool, and a 208 MiB device window (plus the octree file's sample window for
+// the octree source), kept until simlod_destroy.
+int simlod_write_las(SimlodContext* ctx, const char* path, const SimlodLasWriteParams* params, uint64_t samples,
+                     uint64_t num_samples, int32_t depth, SimlodLasWriteInfo* info, float* kernel_ms);
+// The union box of a list of .las / .simlod files as simlod_insert_files computes it (float header bounds), with the
+// same validation and errors; an octree built from the list holds its points at (world - box_min). No context, no GPU.
+int simlod_files_box(const char* const* paths, uint32_t num_paths, float box_min[3], float box_max[3]);
+
 // Raw access for tests and tools: device addresses and sizes of the buffers the kernels share
 // (nodes[], persistent heap, momentary buffer, render buffer, point ring) and a bounded copy.
 typedef struct SimlodBuffers {

@@ -9,4 +9,4 @@ Only what the path needs lives here:
   data.py     synthetic point streams of the benchmark configurations
   dist.py     batch sharding + reductions for one-process-per-GPU insertion
 """
-from .api import SimLOD, SimlodError, make_points, POINT_DTYPE, load_library, read_las_header, Region  # noqa: F401
+from .api import SimLOD, SimlodError, make_points, POINT_DTYPE, load_library, read_las_header, Region, files_box  # noqa: F401

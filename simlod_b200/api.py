@@ -194,6 +194,23 @@ class SimlodRadiusInfo(C.Structure):
                 ("count_ms", C.c_float), ("write_ms", C.c_float)]
 
 
+class LasWriteParams(C.Structure):
+    """SimlodLasWriteParams: the file's scale and offset, the translation added to every sample, the writer threads."""
+    _fields_ = [("scale", C.c_double * 3), ("offset", C.c_double * 3), ("translation", C.c_double * 3),
+                ("writer_threads", C.c_uint32), ("reserved", C.c_uint32)]
+
+
+class LasWriteInfo(C.Structure):
+    """SimlodLasWriteInfo: records written, file size, the first invalid sample (UINT64_MAX for none), the header's
+    bounds, and the time of each stage."""
+    _fields_ = [("num_points", C.c_uint64), ("file_size", C.c_uint64), ("first_invalid", C.c_uint64),
+                ("min", C.c_double * 3), ("max", C.c_double * 3), ("plan_ms", C.c_float), ("encode_ms", C.c_float),
+                ("copy_ms", C.c_float), ("write_ms", C.c_float), ("num_windows", C.c_uint32), ("reserved", C.c_uint32)]
+
+
+NO_INVALID = (1 << 64) - 1
+
+
 class Region:
     """Constructors of the regions SimLOD.query_region takes. Numbers are rounded to float32, the type the predicates are
     evaluated in; a malformed region (non-finite number, min > max, negative radius) is refused by the query."""
@@ -240,6 +257,7 @@ assert C.sizeof(OctreeFileHeader) == 128
 assert C.sizeof(SimlodRegion) == 304 and C.sizeof(SimlodQueryInfo) == 40
 assert C.sizeof(SimlodPickInfo) == 40 and C.sizeof(SimlodNearestInfo) == 64 and C.sizeof(SimlodRayInfo) == 56
 assert C.sizeof(SimlodRadiusInfo) == 64
+assert C.sizeof(LasWriteParams) == 80 and C.sizeof(LasWriteInfo) == 96
 
 # every symbol include/simlod_b200.h declares
 EXPORTS = [
@@ -253,7 +271,7 @@ EXPORTS = [
     "simlod_export_framebuffer", "simlod_peer_signal", "simlod_composite_framebuffers", "simlod_generate", "simlod_reset_with_grid", "simlod_insert_simlod_file_ex", "simlod_get_numa_node",
     "simlod_export_octree", "simlod_export_view", "simlod_read_las_header", "simlod_insert_files",
     "simlod_read_octree_header", "simlod_save_octree", "simlod_load_octree", "simlod_query_region",
-    "simlod_pick", "simlod_query_nearest", "simlod_query_ray", "simlod_query_radius",
+    "simlod_pick", "simlod_query_nearest", "simlod_query_ray", "simlod_query_radius", "simlod_write_las", "simlod_files_box",
 ]
 
 _lib = None
@@ -323,6 +341,9 @@ def load_library():
         "simlod_query_ray": [vp, u64, u64, C.c_float, C.c_int32, u64, u64, u64, u64, C.POINTER(SimlodRayInfo), C.POINTER(C.c_float)],
         "simlod_query_radius": [vp, u64, u64, C.c_float, C.c_int32, u64, u64, u64, u64, u64, C.POINTER(SimlodRadiusInfo),
                                 C.POINTER(C.c_float)],
+        "simlod_write_las": [vp, C.c_char_p, C.POINTER(LasWriteParams), u64, u64, C.c_int32, C.POINTER(LasWriteInfo),
+                             C.POINTER(C.c_float)],
+        "simlod_files_box": [C.POINTER(C.c_char_p), u32, C.POINTER(C.c_float), C.POINTER(C.c_float)],
     }
     for name, argtypes in sig.items():
         fn = getattr(lib, name)
@@ -352,6 +373,32 @@ def read_octree_header(path):
     if rc != 0:
         raise SimlodError(rc, lib.simlod_last_error().decode())
     return h
+
+
+def files_box(paths):
+    """The union box (box_min, box_max) of a list of .las / .simlod files, as SimLOD.insert_files computes it from their
+    headers (simlod_files_box), with the same validation and errors. insert_files stores a point at world - box_min, so
+    write_las(..., translation=box_min) puts an octree built from the list back at its world position. Needs no GPU."""
+    lib = load_library()
+    enc = [os.fsencode(p) for p in paths]
+    arr = (C.c_char_p * max(1, len(enc)))(*enc)
+    mn, mx = (C.c_float * 3)(), (C.c_float * 3)()
+    rc = lib.simlod_files_box(arr, len(enc), mn, mx)
+    if rc != 0:
+        raise SimlodError(rc, lib.simlod_last_error().decode())
+    return np.array(mn[:], dtype=np.float32), np.array(mx[:], dtype=np.float32)
+
+
+def las_write_params(scale=0.001, offset=None, translation=(0.0, 0.0, 0.0), writer_threads=8):
+    """SimlodLasWriteParams from a scalar or 3-tuple scale, an offset (None: the translation) and a translation."""
+    sc = [float(scale)] * 3 if np.ndim(scale) == 0 else [float(v) for v in scale]
+    tr = [float(v) for v in translation]
+    of = tr if offset is None else [float(v) for v in offset]
+    if len(sc) != 3 or len(tr) != 3 or len(of) != 3:
+        raise ValueError("scale, offset and translation take 3 values (a scalar scale applies to every axis)")
+    p = LasWriteParams(writer_threads=int(writer_threads))
+    p.scale[:], p.offset[:], p.translation[:] = sc, of, tr
+    return p
 
 
 def make_points(xyz, color):
@@ -558,6 +605,61 @@ class SimLOD:
         self._lib.simlod_get_uniforms(self._ctx, C.byref(self.uniforms))
         self._check(rc)
         return info, ms.value
+
+    def write_las_into(self, path, params, samples_ptr, num_samples, depth):
+        """simlod_write_las with SimlodLasWriteParams: samples_ptr 0 for the octree source (depth None or < 0: the
+        inserted points), else num_samples 16-byte samples at a 16-byte aligned device address. Returns (LasWriteInfo,
+        kernel ms); on SimlodError the info is the exception's `.info` (first_invalid names an invalid sample)."""
+        info, ms = LasWriteInfo(), C.c_float(0)
+        d = -1 if depth is None else int(depth)
+        rc = self._lib.simlod_write_las(self._ctx, os.fsencode(path), C.byref(params), int(samples_ptr), int(num_samples), d,
+                                        C.byref(info), C.byref(ms))
+        if rc != 0:
+            err = SimlodError(rc, self._lib.simlod_last_error().decode())
+            err.info = info
+            raise err
+        return info, ms.value
+
+    def write_las(self, path, samples=None, depth=None, scale=0.001, offset=None, translation=(0.0, 0.0, 0.0), writer_threads=8):
+        """Write samples to a LAS 1.2 file (point format 2), quantised and encoded on the GPU (simlod_write_las).
+
+        Record i of the file is sample i of the source: of `samples`, or with samples=None of
+        export_octree(depth).samples for the octree as the last completed update left it (depth=None: the inserted
+        points, export_octree(20), those on the cube's max face included). `samples`: a CUDA float32 (N, 4) tensor (x, y,
+        z, colour bits; used in place when contiguous and 16-byte aligned), or a numpy POINT_DTYPE or (N, 4) float32
+        array (copied to the device) -- the layout export_*, query_region and the queries' samples=True return.
+        Per axis, in IEEE double: q = rint(((double(p) + translation) - offset) / scale), half to even, with offset
+        defaulting to translation, so a reader sees x = q * scale + offset near p + translation. `scale` is a scalar or
+        a 3-tuple. A non-finite coordinate or a q outside int32 refuses the call, naming the first such sample in
+        SimlodError.info.first_invalid; a failed call leaves no file and an existing file at `path` as it was.
+        Colours become R, G, B = 257 * colour byte (alpha dropped). Returns the LasWriteInfo."""
+        params = las_write_params(scale, offset, translation, writer_threads)
+        if samples is None:
+            return self.write_las_into(path, params, 0, 0, depth)[0]
+        if not isinstance(samples, np.ndarray) and hasattr(samples, "data_ptr"):
+            import torch
+            if not samples.is_cuda or samples.dtype != torch.float32 or samples.ndim != 2 or samples.shape[1] != 4:
+                raise ValueError("samples must be a CUDA float32 (N, 4) tensor, or a POINT_DTYPE or (N, 4) float32 array")
+            t = samples if samples.is_contiguous() and samples.data_ptr() % 16 == 0 else samples.contiguous().clone()
+            torch.cuda.current_stream(t.device).synchronize()   # the samples may still be being computed on torch's stream
+            n = t.shape[0]
+            if n and t.data_ptr():
+                return self.write_las_into(path, params, t.data_ptr(), n, depth)[0]
+            a = np.zeros((0, 4), dtype=np.float32)
+        else:
+            a = np.asarray(samples)
+            if a.dtype == POINT_DTYPE:
+                a = a.reshape(-1).view(np.float32).reshape(-1, 4)
+            if a.dtype != np.float32 or a.ndim != 2 or a.shape[1] != 4:
+                raise ValueError("samples must be a CUDA float32 (N, 4) tensor, or a POINT_DTYPE or (N, 4) float32 array")
+            a = np.ascontiguousarray(a)
+        dptr = self.device_alloc(max(a.nbytes, 16))           # an empty array still needs an address: 0 is the octree
+        try:
+            if a.nbytes:
+                self.memcpy_htod(dptr, a)
+            return self.write_las_into(path, params, dptr, a.shape[0], depth)[0]
+        finally:
+            self.device_free(dptr)
 
     def insert_batches(self, batches):
         """Insert explicit batches (each <= 1 M points), each followed by update launches until the

@@ -52,6 +52,7 @@ extern const unsigned char simlod_cubin_pick[];
 extern const unsigned char simlod_cubin_nearest[];
 extern const unsigned char simlod_cubin_ray[];
 extern const unsigned char simlod_cubin_radius[];
+extern const unsigned char simlod_cubin_las_write[];
 }
 
 namespace {
@@ -117,10 +118,10 @@ struct Program {
 
 // The embedded images of the kernels that are launched outside the three swappable programs, and those kernels: one
 // row each, {enum value, image, kernel name}. createResources loads every image and looks up every kernel.
-enum Image { IMG_UTIL, IMG_LAS, IMG_GEN, IMG_PARTITION, IMG_EXPORT, IMG_QUERY, IMG_IMPORT, IMG_PICK, IMG_NEAREST, IMG_RAY, IMG_RADIUS, NUM_IMAGES };
+enum Image { IMG_UTIL, IMG_LAS, IMG_GEN, IMG_PARTITION, IMG_EXPORT, IMG_QUERY, IMG_IMPORT, IMG_PICK, IMG_NEAREST, IMG_RAY, IMG_RADIUS, IMG_LAS_WRITE, NUM_IMAGES };
 const unsigned char* const IMAGES[NUM_IMAGES] = {simlod_cubin_util, simlod_cubin_las, simlod_cubin_gen, simlod_cubin_partition,
                                                  simlod_cubin_export, simlod_cubin_query, simlod_cubin_import, simlod_cubin_pick,
-                                                 simlod_cubin_nearest, simlod_cubin_ray, simlod_cubin_radius};
+                                                 simlod_cubin_nearest, simlod_cubin_ray, simlod_cubin_radius, simlod_cubin_las_write};
 #define KERNEL_LIST(X)                                                                                    \
     X(K_RCP, IMG_UTIL, "simlod_util_rcp") X(K_FILL, IMG_UTIL, "simlod_util_fill")                         \
     X(K_LAS, IMG_LAS, "simlod_las_decode")                                                                \
@@ -144,7 +145,8 @@ const unsigned char* const IMAGES[NUM_IMAGES] = {simlod_cubin_util, simlod_cubin
     X(K_NEAREST_SCATTER, IMG_NEAREST, "simlod_nearest_scatter") X(K_NEAREST_SEARCH, IMG_NEAREST, "simlod_nearest_search") \
     X(K_RAY_CHECK, IMG_RAY, "simlod_ray_check") X(K_RAY_TRACE, IMG_RAY, "simlod_ray_trace")                 \
     X(K_RADIUS_COUNT, IMG_RADIUS, "simlod_radius_count") X(K_RADIUS_REDUCE, IMG_RADIUS, "simlod_radius_reduce") \
-    X(K_RADIUS_SCAN, IMG_RADIUS, "simlod_radius_scan") X(K_RADIUS_WRITE, IMG_RADIUS, "simlod_radius_write")
+    X(K_RADIUS_SCAN, IMG_RADIUS, "simlod_radius_scan") X(K_RADIUS_WRITE, IMG_RADIUS, "simlod_radius_write") \
+    X(K_LAS_ENCODE, IMG_LAS_WRITE, "simlod_las_encode")
 #define X(k, image, name) k,
 enum Kernel { KERNEL_LIST(X) NUM_KERNELS };
 #undef X
@@ -217,6 +219,8 @@ struct SimlodContext {
     uint64_t rayCtlBytes = 0;
     CUdeviceptr fileWindow = 0;        // octree files: FILE_WINDOW_BYTES of samples staged on the device
     CUdeviceptr fileTables = 0;        // octree load: records | plan | error word, sized for nodes[]
+    CUdeviceptr lasWindow = 0;         // LAS writer: one window of records, then LasWriteCtl
+    CUevent evLas[2][4] = {};          // LAS writer, per pool half: encode start, encode end, copy start, records copied out
     uint64_t fileTablesBytes = 0;
     void* pinnedPool = nullptr;        // POOL_BYTES page-locked: the file streamer's slots, one batch of records each
     LoaderPool* loaderPool = nullptr;
@@ -635,6 +639,8 @@ void simlod_destroy(SimlodContext* ctx) {
         if (ctx->rayCtl) D(cuMemFree)(ctx->rayCtl);
         if (ctx->fileWindow) D(cuMemFree)(ctx->fileWindow);
         if (ctx->fileTables) D(cuMemFree)(ctx->fileTables);
+        if (ctx->lasWindow) D(cuMemFree)(ctx->lasWindow);
+        for (auto& half : ctx->evLas) for (CUevent e : half) if (e) D(cuEventDestroy)(e);
         delete ctx->loaderPool;          // joins the loader threads
         if (ctx->pinnedPool) D(cuMemFreeHost)(ctx->pinnedPool);
         for (int i = 0; i < 32; i++) if (ctx->evPool[i]) D(cuEventDestroy)(ctx->evPool[i]);
@@ -1089,6 +1095,25 @@ int openForStream(StreamFile* f, bool direct) {
     return SIMLOD_OK;
 }
 
+// One entry of a file list: the path must exist and name a .las or .simlod file, whose header is read and checked
+int probeListedFile(const char* p, uint32_t i, StreamFile* f) {
+    if (!p) return fail(SIMLOD_ERR_INVALID, "null path at list position %u", i);
+    struct stat st;
+    if (stat(p, &st) != 0) return fail(SIMLOD_ERR_INVALID, "%s does not exist", p);
+    const std::string s(p);
+    if (iEndsWith(s, ".laz")) return fail(SIMLOD_ERR_INVALID, "%s: LAZ is not supported", p);
+    if (iEndsWith(s, ".las")) return probeLas(p, f);
+    if (iEndsWith(s, ".simlod")) return probeSimlod(p, f);
+    return fail(SIMLOD_ERR_INVALID, "%s: unsupported file type (expected .las or .simlod)", p);
+}
+
+// the union of the files' boxes (main.cpp:700-709, 724-733, 763-765)
+void unionBox(const StreamFiles& files, float bmin[3], float bmax[3]) {
+    for (int i = 0; i < 3; i++) { bmin[i] = std::numeric_limits<float>::infinity(); bmax[i] = -bmin[i]; }
+    for (const StreamFile& f : files.v)
+        for (int a = 0; a < 3; a++) { bmin[a] = std::min(bmin[a], f.min[a]); bmax[a] = std::max(bmax[a], f.max[a]); }
+}
+
 }  // namespace
 
 extern "C" {
@@ -1098,13 +1123,12 @@ extern "C" {
 static int streamFiles(SimlodContext* ctx, StreamFiles& files, int loader_threads, uint64_t* num_points, float* kernel_ms, float* total_ms) {
     // the box (main.cpp:700-709, 724-733, 763-765) and the batch list (main.cpp:711-720, 737-745)
     float bmin[3], bmax[3];
-    for (int i = 0; i < 3; i++) { bmin[i] = std::numeric_limits<float>::infinity(); bmax[i] = -bmin[i]; }
+    unionBox(files, bmin, bmax);
     std::vector<StreamBatch> batches;
     uint64_t numPoints = 0;
     uint32_t maxBpp = 0, maxLasBpp = 0;
     for (uint32_t i = 0; i < (uint32_t)files.v.size(); i++) {
         const StreamFile& f = files.v[i];
-        for (int a = 0; a < 3; a++) { bmin[a] = std::min(bmin[a], f.min[a]); bmax[a] = std::max(bmax[a], f.max[a]); }
         for (uint64_t first = 0; first < f.numPoints; first += SLOT_POINTS)
             batches.push_back({i, first, (uint32_t)std::min<uint64_t>(SLOT_POINTS, f.numPoints - first)});
         numPoints += f.numPoints;
@@ -1275,20 +1299,21 @@ int simlod_insert_files(SimlodContext* ctx, const char* const* paths, uint32_t n
     StreamFiles files;
     files.v.resize(num_paths);
     for (uint32_t i = 0; i < num_paths; i++) {
-        const char* p = paths[i];
-        if (!p) return fail(SIMLOD_ERR_INVALID, "null path at list position %u", i);
-        struct stat st;
-        if (stat(p, &st) != 0) return fail(SIMLOD_ERR_INVALID, "%s does not exist", p);
-        const std::string s(p);
-        if (iEndsWith(s, ".laz")) rc = fail(SIMLOD_ERR_INVALID, "%s: LAZ is not supported", p);
-        else if (iEndsWith(s, ".las")) rc = probeLas(p, &files.v[i]);
-        else if (iEndsWith(s, ".simlod")) rc = probeSimlod(p, &files.v[i]);
-        else rc = fail(SIMLOD_ERR_INVALID, "%s: unsupported file type (expected .las or .simlod)", p);
-        if (rc) return rc;
+        rc = probeListedFile(paths[i], i, &files.v[i]); if (rc) return rc;
         rc = openForStream(&files.v[i], (flags & SIMLOD_STREAM_DIRECT) != 0); if (rc) return rc;
     }
     rc = setCurrent(ctx); if (rc) return rc;
     return streamFiles(ctx, files, loader_threads, num_points, kernel_ms, total_ms);
+}
+
+int simlod_files_box(const char* const* paths, uint32_t num_paths, float box_min[3], float box_max[3]) {
+    if (!paths || num_paths == 0) return fail(SIMLOD_ERR_INVALID, "empty file list");
+    if (!box_min || !box_max) return fail(SIMLOD_ERR_INVALID, "null argument");
+    StreamFiles files;
+    files.v.resize(num_paths);
+    for (uint32_t i = 0; i < num_paths; i++) { int rc = probeListedFile(paths[i], i, &files.v[i]); if (rc) return rc; }
+    unionBox(files, box_min, box_max);
+    return SIMLOD_OK;
 }
 
 int simlod_render(SimlodContext* ctx, float* kernel_ms) {
@@ -2296,9 +2321,219 @@ int loadOctree(SimlodContext* ctx, const char* path, int loader_threads, SimlodE
     if (kernel_ms) *kernel_ms = ms;
     return SIMLOD_OK;
 }
+
+// ---- LAS writer (DESIGN.md §9.13); the encode is las_write.cu's, the octree source's gather export.cu's --------------
+constexpr uint64_t LAS_HEADER_BYTES = 227;                                  // LAS 1.2 public header, no VLRs
+constexpr uint64_t LAS_WINDOW_BYTES = LAS_WRITE_WINDOW * LAS_WRITE_RECORD;  // 208 MiB of records
+constexpr uint64_t LAS_PIECE_BYTES = 8ull << 20;                            // a writer thread's unit of work
+static_assert(LAS_WINDOW_BYTES <= POOL_BYTES / 2, "a window of records fits one half of the page-locked pool");
+static_assert(LAS_WRITE_WINDOW * sizeof(SimlodPoint) <= FILE_WINDOW_BYTES, "a window of samples fits the octree file's window");
+static_assert(2 * sizeof(LasWriteCtl) <= CTL_HOST_BYTES, "two control snapshots fit the pinned control word");
+
+int ensureLasWindow(SimlodContext* ctx) {
+    if (!ctx->lasWindow) {
+        for (auto& half : ctx->evLas) for (CUevent& e : half) if (!e) CU(D(cuEventCreate)(&e, CU_EVENT_DEFAULT));
+        CU(D(cuMemAlloc)(&ctx->lasWindow, LAS_WINDOW_BYTES + sizeof(LasWriteCtl)));
+    }
+    if (!ctx->hExportCtl) CU(D(cuMemHostAlloc)(&ctx->hExportCtl, CTL_HOST_BYTES, 0));
+    return ensurePinnedPool(ctx);
+}
+
+bool pwriteAll(int fd, const char* src, uint64_t bytes, uint64_t at) {
+    while (bytes) {
+        const ssize_t r = pwrite(fd, src, bytes, (off_t)at);
+        if (r <= 0) return false;
+        src += r; at += (uint64_t)r; bytes -= (uint64_t)r;
+    }
+    return true;
+}
+
+void lasHeader(uint8_t* h, uint64_t n, const SimlodLasWriteParams& p, const double mn[3], const double mx[3]) {
+    memset(h, 0, LAS_HEADER_BYTES);
+    auto u16 = [&](int o, uint16_t v) { memcpy(h + o, &v, 2); };
+    auto u32 = [&](int o, uint32_t v) { memcpy(h + o, &v, 4); };
+    auto f64 = [&](int o, double v) { memcpy(h + o, &v, 8); };
+    memcpy(h, "LASF", 4);
+    h[24] = 1; h[25] = 2;                                   // version 1.2; system identifier zero bytes
+    memcpy(h + 58, "simlod_b200", 11);                      // generating software, NUL-padded; creation day and year 0
+    u16(94, (uint16_t)LAS_HEADER_BYTES);
+    u32(96, (uint32_t)LAS_HEADER_BYTES);                    // offset to point data; 0 VLRs
+    h[104] = 2;
+    u16(105, (uint16_t)LAS_WRITE_RECORD);
+    u32(107, (uint32_t)n);
+    u32(111, (uint32_t)n);                                  // points by return [n, 0, 0, 0, 0]
+    for (int a = 0; a < 3; a++) {
+        f64(131 + 8 * a, p.scale[a]);
+        f64(155 + 8 * a, p.offset[a]);
+        f64(179 + 16 * a, mx[a]);
+        f64(187 + 16 * a, mn[a]);
+    }
+}
+
+int writeLas(SimlodContext* ctx, const char* path, const SimlodLasWriteParams* params, uint64_t samples, uint64_t numSamples,
+             int32_t depth, SimlodLasWriteInfo* info, float* kernel_ms) {
+    int rc = setCurrent(ctx); if (rc) return rc;
+    if (!path || !params || !info) return fail(SIMLOD_ERR_INVALID, "null path, params or info");
+    for (int a = 0; a < 3; a++) {
+        if (!std::isfinite(params->scale[a]) || !(params->scale[a] > 0.0)) return fail(SIMLOD_ERR_INVALID, "LAS scale[%d] = %g must be finite and > 0", a, params->scale[a]);
+        if (!std::isfinite(params->offset[a]) || !std::isfinite(params->translation[a])) return fail(SIMLOD_ERR_INVALID, "LAS offset and translation must be finite (axis %d)", a);
+    }
+    if (samples % 16) return fail(SIMLOD_ERR_INVALID, "samples must be 16-byte aligned");
+    if (samples && depth >= 0) return fail(SIMLOD_ERR_INVALID, "a depth selects a cut of the octree's samples; it does not apply to a caller's array");
+    if (depth > SIMLOD_MAX_DEPTH) return fail(SIMLOD_ERR_INVALID, "LAS depth %d exceeds the octree's maximum depth %d", depth, (int)SIMLOD_MAX_DEPTH);
+    if (samples && numSamples > UINT32_MAX) return fail(SIMLOD_ERR_INVALID, "%llu samples: a LAS 1.2 file holds at most 2^32 - 1 points", (unsigned long long)numSamples);
+    if (params->writer_threads < 1 || params->writer_threads > 64) return fail(SIMLOD_ERR_INVALID, "writer_threads %u is outside 1..64", params->writer_threads);
+    // written under a temporary name and renamed once complete: a failed call leaves no file and replaces no existing one
+    const std::string tmpPath = std::string(path) + ".tmp";
+    int fd = open(tmpPath.c_str(), O_WRONLY | O_CREAT | O_TRUNC | O_CLOEXEC, 0644);
+    if (fd < 0) return fail(SIMLOD_ERR_INVALID, "cannot write %s", path);
+    struct Closer {
+        int& fd; const std::string& tmp; bool done = false;
+        ~Closer() { if (fd >= 0) close(fd); if (!done) unlink(tmp.c_str()); }
+    } closer{fd, tmpPath};
+    memset(info, 0, sizeof(*info));
+    info->first_invalid = UINT64_MAX;
+
+    // the octree source: the export's plan and chunk-list walk, once
+    const bool octree = samples == 0;
+    ExportPlanned p;
+    uint64_t n = numSamples;
+    if (octree) {
+        rc = exportPlan(ctx, depth < 0 ? (int32_t)SIMLOD_MAX_DEPTH : depth, nullptr, &p);
+        info->plan_ms = p.ms;
+        if (rc) return fail(rc, "%s: not written: %s", path, g_error.c_str());
+        n = p.c.numSamples;
+        if (n > UINT32_MAX) return fail(SIMLOD_ERR_INVALID, "%s: not written: %llu samples, a LAS 1.2 file holds at most 2^32 - 1 points", path, (unsigned long long)n);
+        rc = ensureFileWindow(ctx); if (rc) return rc;
+    }
+    rc = ensureLasWindow(ctx); if (rc) return rc;
+    const uint64_t fileSize = LAS_HEADER_BYTES + n * LAS_WRITE_RECORD;
+    if (ftruncate(fd, (off_t)fileSize) != 0) return fail(SIMLOD_ERR_INVALID, "write error in %s", path);
+
+    // window w: gathered (octree source) and encoded on the device, copied into pool half w & 1 with its control
+    // snapshot; its pieces are handed to the writers once the copy has completed and shows no invalid sample
+    const uint64_t numWindows = (n + LAS_WRITE_WINDOW - 1) / LAS_WRITE_WINDOW;
+    auto windowCount = [&](uint64_t w) { return std::min<uint64_t>(LAS_WRITE_WINDOW, n - w * LAS_WRITE_WINDOW); };
+    auto half = [&](uint64_t w) { return (char*)ctx->pinnedPool + (w & 1) * (POOL_BYTES / 2); };
+    std::vector<uint64_t> firstPiece(numWindows + 1, 0);          // pieces of windows [0, w)
+    for (uint64_t w = 0; w < numWindows; w++)
+        firstPiece[w + 1] = firstPiece[w] + (windowCount(w) * LAS_WRITE_RECORD + LAS_PIECE_BYTES - 1) / LAS_PIECE_BYTES;
+    const uint64_t totalPieces = firstPiece[numWindows];
+    std::vector<std::atomic<uint64_t>> written(numWindows);       // pieces of window w in the file
+    for (auto& c : written) c.store(0);
+    std::atomic<uint64_t> published{0}, nextPiece{0};             // pieces [0, published) may be written
+    std::atomic<bool> abort{false}, ioError{false};
+    if (!ctx->loaderPool) ctx->loaderPool = new LoaderPool();
+    LoaderPool* pool = ctx->loaderPool;
+    const auto tBegin = std::chrono::steady_clock::now();
+    pool->run((int)params->writer_threads, [&](int) {
+        for (;;) {
+            const uint64_t item = nextPiece.fetch_add(1);
+            if (item >= totalPieces) break;
+            while (published.load() <= item && !abort.load()) std::this_thread::yield();
+            if (abort.load()) break;
+            const uint64_t w = (uint64_t)(std::upper_bound(firstPiece.begin(), firstPiece.end(), item) - firstPiece.begin()) - 1;
+            const uint64_t bytes = windowCount(w) * LAS_WRITE_RECORD, p0 = (item - firstPiece[w]) * LAS_PIECE_BYTES;
+            const uint64_t at = LAS_HEADER_BYTES + w * LAS_WINDOW_BYTES + p0;
+            if (!pwriteAll(fd, half(w) + p0, std::min<uint64_t>(LAS_PIECE_BYTES, bytes - p0), at)) { ioError.store(true); abort.store(true); break; }
+            written[w].fetch_add(1);
+        }
+    });
+    // stops and joins the writers on every exit
+    struct Writers {
+        LoaderPool* pool; std::atomic<bool>& abort; bool joined = false;
+        void join(bool stop) { if (joined) return; if (stop) abort.store(true); pool->wait(); joined = true; }
+        ~Writers() { join(true); }
+    } writers{pool, abort};
+    const LasWriteCtl* hctl = (const LasWriteCtl*)ctx->hExportCtl;
+    const CUdeviceptr records = ctx->lasWindow, ctl = ctx->lasWindow + LAS_WINDOW_BYTES;
+    CU(D(cuMemsetD8Async)(ctl, 0xff, sizeof(LasWriteCtl), ctx->streamMain));
+    float encodeMs = 0.0f, copyMs = 0.0f;
+    auto drain = [&](uint64_t w) -> int {             // window w has been copied out: time it, check it, publish it
+        CUevent* ev = ctx->evLas[w & 1];
+        CU(D(cuEventSynchronize)(ev[3]));
+        float e = 0.0f, c = 0.0f;
+        CU(D(cuEventElapsedTime)(&e, ev[0], ev[1]));
+        CU(D(cuEventElapsedTime)(&c, ev[2], ev[3]));
+        encodeMs += e; copyMs += c;
+        if (hctl[w & 1].firstInvalid != UINT64_MAX) {
+            info->first_invalid = hctl[w & 1].firstInvalid;
+            return fail(SIMLOD_ERR_INVALID, "%s: not written: sample %llu is invalid (a non-finite coordinate, or a quantised coordinate outside int32)",
+                        path, (unsigned long long)info->first_invalid);
+        }
+        published.store(firstPiece[w + 1]);
+        return SIMLOD_OK;
+    };
+    const unsigned maxBlocks = (unsigned)ctx->numSMs * 8;
+    for (uint64_t w = 0; w < numWindows; w++) {
+        const uint64_t a = w * LAS_WRITE_WINDOW, count = windowCount(w);
+        CUevent* ev = ctx->evLas[w & 1];
+        CU(D(cuEventRecord)(ev[0], ctx->streamMain));
+        CUdeviceptr src = (CUdeviceptr)samples + a * sizeof(SimlodPoint);
+        if (octree) {
+            CUdeviceptr window = ctx->fileWindow;
+            uint64_t b = a + count;
+            rc = launch(ctx, ctx->fn[K_EXPORT_GATHER_WINDOW], (unsigned)ctx->numSMs * 4, 256, ctx->streamMain, p.s.items, window, p.s.ctl, a, b);
+            if (rc) return rc;
+            src = window;
+        }
+        LasEncodeArgs args{devPtr(src), devPtr(records), devPtr(ctl), a, count, {}, {}, {}};
+        for (int k = 0; k < 3; k++) { args.scale[k] = params->scale[k]; args.offset[k] = params->offset[k]; args.translation[k] = params->translation[k]; }
+        const unsigned grid = (unsigned)std::min<uint64_t>(maxBlocks, (count + LAS_WRITE_TILE - 1) / LAS_WRITE_TILE);
+        rc = launch(ctx, ctx->fn[K_LAS_ENCODE], grid, LAS_WRITE_TILE, ctx->streamMain, args); if (rc) return rc;
+        CU(D(cuEventRecord)(ev[1], ctx->streamMain));
+        // pool half w & 1 is free once every piece of window w - 2 is in the file
+        if (w >= 2) {
+            while (written[w - 2].load() < firstPiece[w - 1] - firstPiece[w - 2] && !abort.load()) std::this_thread::yield();
+            if (ioError.load()) return fail(SIMLOD_ERR_INVALID, "write error in %s", path);
+        }
+        CU(D(cuEventRecord)(ev[2], ctx->streamMain));
+        CU(D(cuMemcpyDtoHAsync)(half(w), records, (size_t)(count * LAS_WRITE_RECORD), ctx->streamMain));
+        CU(D(cuMemcpyDtoHAsync)((void*)(hctl + (w & 1)), ctl, sizeof(LasWriteCtl), ctx->streamMain));
+        CU(D(cuEventRecord)(ev[3], ctx->streamMain));
+        if (w > 0) { rc = drain(w - 1); if (rc) return rc; }
+    }
+    if (numWindows > 0) { rc = drain(numWindows - 1); if (rc) return rc; }
+    writers.join(false);
+    if (ioError.load()) return fail(SIMLOD_ERR_INVALID, "write error in %s", path);
+
+    // the header last, once the bounds are known: double(q) * scale + offset, multiply then add
+    double mn[3] = {0.0, 0.0, 0.0}, mx[3] = {0.0, 0.0, 0.0};
+    if (n > 0) {
+        const LasWriteCtl& c = hctl[(numWindows - 1) & 1];
+        for (int a = 0; a < 3; a++) {
+            const int32_t qmin = (int32_t)(c.qmin[a] ^ 0x80000000u), qmax = (int32_t)(~c.qmaxInv[a] ^ 0x80000000u);
+            volatile double lo = (double)qmin * params->scale[a], hi = (double)qmax * params->scale[a];   // no contraction
+            mn[a] = lo + params->offset[a];
+            mx[a] = hi + params->offset[a];
+        }
+    }
+    uint8_t head[LAS_HEADER_BYTES];
+    lasHeader(head, n, *params, mn, mx);
+    if (!pwriteAll(fd, (const char*)head, LAS_HEADER_BYTES, 0)) return fail(SIMLOD_ERR_INVALID, "write error in %s", path);
+    const int closed = close(fd);
+    fd = -1;
+    if (closed != 0) return fail(SIMLOD_ERR_INVALID, "write error in %s", path);
+    if (rename(tmpPath.c_str(), path) != 0) return fail(SIMLOD_ERR_INVALID, "cannot write %s (rename from %s failed)", path, tmpPath.c_str());
+    closer.done = true;
+    info->num_points = n;
+    info->file_size = fileSize;
+    for (int a = 0; a < 3; a++) { info->min[a] = mn[a]; info->max[a] = mx[a]; }
+    info->encode_ms = encodeMs;
+    info->copy_ms = copyMs;
+    info->write_ms = (float)std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - tBegin).count();
+    info->num_windows = (uint32_t)numWindows;
+    if (kernel_ms) *kernel_ms = info->plan_ms + encodeMs;
+    return SIMLOD_OK;
+}
 }  // namespace
 
 extern "C" {
+
+int simlod_write_las(SimlodContext* ctx, const char* path, const SimlodLasWriteParams* params, uint64_t samples,
+                     uint64_t num_samples, int32_t depth, SimlodLasWriteInfo* info, float* kernel_ms) {
+    return writeLas(ctx, path, params, samples, num_samples, depth, info, kernel_ms);
+}
 
 int simlod_read_octree_header(const char* path, SimlodOctreeFileHeader* out) {
     if (!path || !out) return fail(SIMLOD_ERR_INVALID, "null argument");

@@ -1,6 +1,6 @@
 // kernel_args.h — the argument and control structs that host.cpp fills and the kernels read, with the codes and limits
 // both sides use. One definition for both compilers: plain C++ (no device code), included by host.cpp and by export.cu,
-// query.cu, pick.cu, nearest.cu, radius.cu and ray.cu (through export_common.cuh), import.cu and partition.cu. The static_asserts pin
+// query.cu, pick.cu, nearest.cu, radius.cu and ray.cu (through export_common.cuh), import.cu, partition.cu and las_write.cu. The static_asserts pin
 // every size, and the offsets that one side reads of a struct the other writes, so a layout change fails to compile instead
 // of shifting bytes.
 #pragma once
@@ -158,6 +158,31 @@ struct RayArgs {                          // the export's plan (export scratch),
     float boxMin[3], boxMax[3];           // of the uniforms: the octree cube
 };
 static_assert(sizeof(RayArgs) == 112 && offsetof(RayArgs, numRays) == 72 && offsetof(RayArgs, boxMin) == 88, "RayArgs");
+
+// ---- LAS writer (las_write.cu) ---------------------------------------------------------------------------------------
+
+constexpr uint32_t LAS_WRITE_TILE = 256;                        // samples per block iteration of the encode
+constexpr uint32_t LAS_WRITE_RECORD = 26;                       // bytes of a point-format-2 record
+constexpr uint64_t LAS_WRITE_WINDOW = 8ull << 20;               // samples per window (208 MiB of records)
+
+// Every word is an unsigned minimum, so that one memset of 0xff resets the whole struct once per call: qmin holds
+// q ^ 0x80000000 (signed order as unsigned), qmaxInv holds ~(q ^ 0x80000000). Read back with each window's records.
+struct LasWriteCtl {
+    uint32_t qmin[3], qmaxInv[3];         // over the valid samples of every window encoded so far
+    uint64_t firstInvalid;                // source index of the first invalid sample, UINT64_MAX for none
+    uint64_t pad;
+};
+static_assert(sizeof(LasWriteCtl) == 40 && offsetof(LasWriteCtl, firstInvalid) == 24, "LasWriteCtl");
+
+struct LasEncodeArgs {
+    const SimlodPoint* samples;           // [i] the window's samples, 16-byte aligned
+    uint8_t* records;                     // [i] their 26-byte records, 16-byte aligned
+    LasWriteCtl* ctl;
+    uint64_t first;                       // source index of samples[0]
+    uint64_t count;                       // samples in the window
+    double scale[3], offset[3], translation[3];
+};
+static_assert(sizeof(LasEncodeArgs) == 112 && offsetof(LasEncodeArgs, scale) == 40 && offsetof(LasEncodeArgs, translation) == 88, "LasEncodeArgs");
 
 // ---- octree import (import.cu) ------------------------------------------------------------------------------------
 
