@@ -362,6 +362,17 @@ __device__ __forceinline__ void voxelFlushPatch(const Ctx& c, const Batch& b, bo
 // counts more than ITEM_CAP items); a final slot (table full, counted globally at once) is the plain index.
 constexpr uint32_t PROVISIONAL = 0x80000000u;
 static_assert(scratch::ITEM_CAP < (1u << 24), "block-local ranks must fit 24 bits");
+// Worklist rounds count without the table: every item moves out of one of the round's (at most 64) split leaves, so its
+// new leaf is child `octant` of split k, and a direct counter per child e = k * 8 + octant takes the block's ranks.
+// Their provisional slots name the child: bit 31 | e << 11 | block-local rank (< LIST_CAP: only listed items count here).
+constexpr uint32_t CHILD_RANK_BITS = 11;
+constexpr uint32_t CHILD_SLOTS = 64 * 8;
+__shared__ uint32_t sh_childCount[CHILD_SLOTS];     // the round's counts per child; after the flush, the child's base
+__shared__ uint8_t  sh_childSplit[CHILD_SLOTS];     // split phase: child e of the last round -> 1 + index of its leaf among the round's splits (0: not split)
+__shared__ uint32_t sh_roundSplits;                 // the leaves split in the last worklist round (entries of sh_splitInfo)
+__device__ __forceinline__ uint32_t childWord(uint32_t e, uint32_t rank) { return PROVISIONAL | (e << CHILD_RANK_BITS) | rank; }
+__device__ __forceinline__ uint32_t childOf(uint32_t sl) { return (sl >> CHILD_RANK_BITS) & (CHILD_SLOTS - 1u); }
+__device__ __forceinline__ uint32_t finalChildSlot(uint32_t sl) { return (sl & PROVISIONAL) ? sh_childCount[childOf(sl)] + (sl & ((1u << CHILD_RANK_BITS) - 1u)) : sl; }
 __shared__ uint32_t sh_leafKey[VOXTAB_SIZE];
 __shared__ uint32_t sh_leafCount[VOXTAB_SIZE];
 __shared__ uint32_t sh_leafBase[VOXTAB_SIZE];
@@ -379,6 +390,7 @@ __shared__ uint32_t sh_runSlot[RUNSLOT_CAP];
 // items (list or table full, run too long for sh_runSlot) raises Ctl::Worklist::legacy; the rounds of that batch then
 // scan the affected runs (markAffectedRun), for which the run filters are kept up to date in every case.
 constexpr uint32_t LIST_CAP = 2048;
+static_assert(LIST_CAP <= (1u << CHILD_RANK_BITS), "a child's block-local ranks must fit its slot word");
 __shared__ uint32_t sh_listCount;         // entries of the explicit list (may run past LIST_CAP: overflow)
 __shared__ uint32_t sh_listMode;          // 0: the run (sh_runSlot), 1: the explicit list
 __shared__ uint32_t sh_blockLegacy;       // this block cannot name its items any more in this batch
@@ -552,6 +564,40 @@ __device__ __forceinline__ uint32_t countInto(const Ctx& c, const Batch& b, bool
         if (MIXED_RUNS) {
             const uint64_t leaderBloom = __shfl_sync(peers, (uint64_t)(uintptr_t)bloom, leader);
             if (bloom && (uint64_t)(uintptr_t)bloom != leaderBloom) bloomAdd(bloom, node);
+        }
+    }
+    return slot;
+}
+
+// count in a worklist round: the lanes that move into the same child e (= split * 8 + octant, see childWord) take
+// consecutive ranks from its direct counter; `child` is its node, for the run filters exactly as in countInto. When the
+// block's item list is full (forceGlobal) they take final slots from the child's global counter at once, as in countInto.
+// ONE_SPLIT: every lane's item comes out of the same split leaf, so lanes with equal octant bits are the peers (three
+// ballots); otherwise they are found by a match on e. Warp-collective; returns the lane's slot word.
+template <bool ONE_SPLIT, bool MIXED_RUNS>
+__device__ __forceinline__ uint32_t countChild(bool valid, uint32_t e, uint32_t child, uint32_t level, uint32_t* bloom, bool forceGlobal) {
+    const uint32_t lane = laneId();
+    uint32_t slot = 0;
+    const uint32_t vmask = __ballot_sync(0xffffffffu, valid);
+    uint32_t peers = 0;
+    if (ONE_SPLIT) {
+        const uint32_t b0 = __ballot_sync(0xffffffffu, e & 1u), b1 = __ballot_sync(0xffffffffu, e & 2u), b2 = __ballot_sync(0xffffffffu, e & 4u);
+        peers = vmask & ((e & 1u) ? b0 : ~b0) & ((e & 2u) ? b1 : ~b1) & ((e & 4u) ? b2 : ~b2);
+    }
+    if (valid) {
+        if (!ONE_SPLIT) peers = __match_any_sync(vmask, e);
+        const uint32_t leader = __ffs(peers) - 1;
+        uint32_t r = 0;
+        if (lane == leader) {
+            if (!forceGlobal) r = childWord(e, atomicAdd(&sh_childCount[e], (uint32_t)__popc(peers)));
+            else              { r = countGlobal(child, level, __popc(peers)); sh_blockLegacy = 1; }
+            if (bloom) bloomAdd(bloom, child);
+        }
+        r = __shfl_sync(peers, r, leader);
+        slot = r + __popc(peers & lanemaskLt());
+        if (MIXED_RUNS) {
+            const uint64_t leaderBloom = __shfl_sync(peers, (uint64_t)(uintptr_t)bloom, leader);
+            if (bloom && (uint64_t)(uintptr_t)bloom != leaderBloom) bloomAdd(bloom, child);
         }
     }
     return slot;
@@ -741,19 +787,39 @@ __device__ void buildWorklist(const Ctx& c, const Batch& b, uint32_t spillBegin,
     blockRun(b.size, blockFirst, blockEnd);
     const uint32_t mode = sh_listMode;
     const uint32_t total = mode == 0 ? blockEnd - blockFirst : min(sh_listCount, LIST_CAP);
-    if (threadIdx.x < numSplit) sh_splitNodes[threadIdx.x] = c.spill()[spillBegin + threadIdx.x].node;
     if (threadIdx.x == 0) { sh_wlCount = 0; sh_wlFill = 0; }
-    __syncthreads();
-    if (threadIdx.x < VOXTAB_SIZE) {
-        const uint32_t key = sh_leafKey[threadIdx.x];
-        uint32_t f = 0;
-        if (key != VOXTAB_EMPTY) for (uint32_t j = 0; j < numSplit; j++) f = key == sh_splitNodes[j] ? j + 1u : f;
-        sh_entrySplit[threadIdx.x] = (uint8_t)f;
+    if (mode == 0) {
+        // the first-visit pass counted through the hashed table: match its entries against the round's splits
+        if (threadIdx.x < numSplit) sh_splitNodes[threadIdx.x] = c.spill()[spillBegin + threadIdx.x].node;
+        __syncthreads();
+        if (threadIdx.x < VOXTAB_SIZE) {
+            const uint32_t key = sh_leafKey[threadIdx.x];
+            uint32_t f = 0;
+            if (key != VOXTAB_EMPTY) for (uint32_t j = 0; j < numSplit; j++) f = key == sh_splitNodes[j] ? j + 1u : f;
+            sh_entrySplit[threadIdx.x] = (uint8_t)f;
+        }
+    } else {
+        // the last round counted into the children of its splits (sh_splitInfo, not yet replaced by this round's): a leaf
+        // split now is child e of one of them, or holds none of the block's items
+        for (uint32_t e = threadIdx.x; e < CHILD_SLOTS; e += blockDim.x) sh_childSplit[e] = 0;
+        __syncthreads();
+        if (threadIdx.x < numSplit) {
+            const uint32_t node = c.spill()[spillBegin + threadIdx.x].node;
+            for (uint32_t k = 0; k < sh_roundSplits; k++) {
+                const uint32_t o = node - sh_splitInfo[k].childBase;
+                if (o < 8u) sh_childSplit[k * 8u + o] = (uint8_t)(threadIdx.x + 1u);
+            }
+        }
     }
     __syncthreads();
     const uint32_t* words = mode == 0 ? sh_runSlot : listSlot();
-    auto movedAt = [&](uint32_t k) { const uint32_t word = words[k]; return (word & PROVISIONAL) != 0 && sh_entrySplit[(word >> 24) & (VOXTAB_SIZE - 1)] != 0; };
-    auto wlSplit = [&](uint32_t word) { return (uint32_t)(sh_entrySplit[(word >> 24) & (VOXTAB_SIZE - 1)] - 1u) << WL_SPLIT_SHIFT; };
+    // 1 + the index among the round's splits of the leaf the item's slot word counted it into (0: the leaf was not split)
+    auto splitOf = [&](uint32_t word) -> uint32_t {
+        if ((word & PROVISIONAL) == 0) return 0u;
+        return mode == 0 ? sh_entrySplit[(word >> 24) & (VOXTAB_SIZE - 1)] : sh_childSplit[childOf(word)];
+    };
+    auto movedAt = [&](uint32_t k) { return splitOf(words[k]) != 0; };
+    auto wlSplit = [&](uint32_t word) { return (splitOf(word) - 1u) << WL_SPLIT_SHIFT; };
     uint32_t cnt = 0;
     for (uint32_t k = threadIdx.x; k < total; k += blockDim.x) cnt += movedAt(k) ? 1u : 0u;
     for (int o = 16; o > 0; o >>= 1) cnt += __shfl_xor_sync(0xffffffffu, cnt, o);
@@ -839,7 +905,8 @@ __device__ __forceinline__ void passItems(const Ctx& c, const Batch& b, uint32_t
             const uint32_t perRun = ((b.size + gridDim.x - 1) / gridDim.x + 31u) & ~31u;
             const uint32_t numSplit = spillEnd - spillBegin;                      // <= 64 in worklist rounds
             if (threadIdx.x < numSplit) sh_splitInfo[threadIdx.x] = c.spill()[spillBegin + threadIdx.x];
-            if (threadIdx.x == 0) { sh_listCount = 0; sh_listMode = 1; }          // the list of the previous round has been read (split phase)
+            for (uint32_t e = threadIdx.x; e < CHILD_SLOTS; e += blockDim.x) sh_childCount[e] = 0;
+            if (threadIdx.x == 0) { sh_listCount = 0; sh_listMode = 1; sh_roundSplits = numSplit; }   // the list of the previous round has been read (split phase)
             __syncthreads();
             if (threadIdx.x == 0) {
                 uint32_t run = 0;
@@ -924,11 +991,15 @@ __device__ __forceinline__ void passItems(const Ctx& c, const Batch& b, uint32_t
                         bool forceGlobal;
                         const uint32_t myk = reserve(valid, forceGlobal);
                         const Coords q = quantize(c, pt);
-                        const uint32_t child = childBase + childIndexAt(q, level);
+                        const uint32_t octant = childIndexAt(q, level);
+                        const uint32_t child = childBase + octant;
                         if (SAMPLE && valid) sampleSplitLeaf(grid, q, pt.w, node, level);
                         __syncwarp();
                         uint32_t slot = 0;
-                        if (COUNT) slot = countInto<true>(c, b, valid, child, level + 1, valid && !spilledItem ? c.runBloom() + (i / perRun) * BLOOM_WORDS : nullptr, forceGlobal);
+                        if (COUNT) {
+                            uint32_t* bloom = valid && !spilledItem ? c.runBloom() + (i / perRun) * BLOOM_WORDS : nullptr;
+                            slot = countChild<false, true>(valid, k * 8u + octant, child, level + 1, bloom, forceGlobal);
+                        }
                         if (valid && COUNT) remember(i, child | ((level + 1) << 24), slot, myk, forceGlobal);
                     }
                     eCur = eNext; ptCur = ptNext; eNext = eNext2;
@@ -973,11 +1044,12 @@ __device__ __forceinline__ void passItems(const Ctx& c, const Batch& b, uint32_t
                         bool forceGlobal;
                         const uint32_t myk = reserve(valid, forceGlobal);
                         const Coords q = quantize(c, pt);
-                        const uint32_t child = childBase + childIndexAt(q, level);
+                        const uint32_t octant = childIndexAt(q, level);
+                        const uint32_t child = childBase + octant;
                         if (SAMPLE && valid) sampleSplitLeaf(sh_splitInfo[cur.lo].grid, q, pt.w, node, level);
                         __syncwarp();
                         uint32_t slot = 0;
-                        if (COUNT) slot = countInto(c, b, valid, child, level + 1, nullptr, forceGlobal);
+                        if (COUNT) slot = countChild<true, false>(valid, cur.lo * 8u + octant, child, level + 1, nullptr, forceGlobal);
                         if (valid && COUNT) remember(i, child | ((level + 1) << 24), slot, myk, forceGlobal);
                     }
                     cur = next; ptCur = ptNext;
@@ -1047,7 +1119,14 @@ __device__ __forceinline__ void passItems(const Ctx& c, const Batch& b, uint32_t
 template <bool SAMPLE, bool COUNT, bool FRESH>
 __device__ __forceinline__ void passFlush(const Ctx& c, const Batch& b, uint32_t numSpilled, uint32_t spilledBefore) {
     // (non-FRESH passes: sh_listMode == 1 and no legacy flag means passItems visited the worklist and kept its items in the list)
-    if (COUNT && threadIdx.x < VOXTAB_SIZE) {
+    if (COUNT && !FRESH && sh_roundLegacy == 0) {
+        // worklist round: one global add per child the block counted into, then the counter holds the child's base
+        for (uint32_t e = threadIdx.x; e < sh_roundSplits * 8u; e += blockDim.x) {
+            const uint32_t cnt = sh_childCount[e];
+            if (cnt > 0) sh_childCount[e] = countGlobal(sh_splitInfo[e >> 3].childBase + (e & 7u), sh_splitInfo[e >> 3].level + 1u, cnt);
+        }
+        if (SAMPLE && threadIdx.x >= 128 && threadIdx.x < 128 + VOXTAB_SIZE) voxelFlushEntry(c, b, threadIdx.x - 128);
+    } else if (COUNT && threadIdx.x < VOXTAB_SIZE) {
         uint32_t leaf = sh_leafKey[threadIdx.x], cnt = sh_leafCount[threadIdx.x];
         if (leaf != VOXTAB_EMPTY && cnt > 0) sh_leafBase[threadIdx.x] = countGlobal(leaf, sh_leafLevel[threadIdx.x], cnt);
     } else if (SAMPLE && threadIdx.x >= 128 && threadIdx.x < 128 + VOXTAB_SIZE) {
@@ -1069,7 +1148,7 @@ __device__ __forceinline__ void passFlush(const Ctx& c, const Batch& b, uint32_t
             const uint32_t n = min(sh_listCount, LIST_CAP);
             const uint32_t* li = listItem();
             const uint32_t* ls = listSlot();
-            for (uint32_t k = threadIdx.x; k < n; k += blockDim.x) if (li[k] != 0xffffffffu) slotOf[li[k]] = finalSlot(ls[k]);
+            for (uint32_t k = threadIdx.x; k < n; k += blockDim.x) if (li[k] != 0xffffffffu) slotOf[li[k]] = finalChildSlot(ls[k]);
         } else {                                                          // ... in the affected runs (legacy rounds)
             const Rewalk rw = rewalkSlice(b.size, numSpilled, spilledBefore);
             for (uint32_t base = rewalkFirstGranule(); base < rw.total; base += rewalkGranuleStride()) {
