@@ -17,6 +17,7 @@ There is no fallback: if libsimlod_b200.so is missing or no H100 is present, con
 """
 import contextlib
 import ctypes as C
+import math
 import os
 
 import numpy as np
@@ -419,6 +420,116 @@ def _as_points(points):
     return a
 
 
+I8, F4 = np.dtype(np.int64), np.dtype(np.float32)
+# numpy dtype of a destination -> (torch dtype, trailing shape) of the tensor that holds it on a CUDA device
+_TORCH_DESTS = {I8: ("int64", ()), F4: ("float32", ()), POINT_DTYPE: ("float32", (4,))}
+
+
+class _Results:
+    """The destinations of one call on `device`, one per (shape, dtype) in `dests` (dtype I8, F4, POINT_DTYPE or
+    EXPORT_NODE_DTYPE; None for one the call does not write). `ptrs` holds their device addresses: 0 for None and for a
+    destination without elements, unless `keep`, which gives each destination at least one row. device="cpu": device
+    memory, freed when the `with` block ends. A CUDA device: torch tensors, and one synchronisation of torch's stream
+    once they are allocated, since the caching allocator may hand out memory torch still uses. results() returns the
+    destinations that are not None, `shape` each: numpy arrays copied out of the device memory, or the tensors
+    (EXPORT_NODE_DTYPE as a numpy array)."""
+    __slots__ = ("_sim", "_dests", "_bufs", "ptrs")
+
+    def __init__(self, sim, device, dests, keep=False):
+        self._sim, self._dests, self._bufs, self.ptrs = sim, dests, None, [0] * len(dests)
+        if device == "cpu":
+            try:
+                for i, d in enumerate(dests):
+                    if d is not None:
+                        nbytes = (max(d[0][0], 1) if keep else d[0][0]) * math.prod(d[0][1:]) * d[1].itemsize
+                        if nbytes:
+                            self.ptrs[i] = sim.device_alloc(nbytes)
+            except BaseException:
+                self.__exit__()
+                raise
+            return
+        import torch
+        dev = torch.device(device)
+        if dev.type != "cuda":
+            raise ValueError("device must be 'cpu' or a CUDA device, not %r" % device)
+        if dev.index is None:
+            dev = torch.device("cuda", sim.device)
+        bufs = self._bufs = [None] * len(dests)
+        for i, d in enumerate(dests):
+            if d is not None:
+                shape, t = d
+                rows = max(shape[0], 1) if keep else shape[0]
+                kind = _TORCH_DESTS.get(t)
+                bufs[i] = (torch.empty((rows,) + shape[1:] + kind[1], dtype=getattr(torch, kind[0]), device=dev) if kind else
+                           torch.empty(rows * t.itemsize, dtype=torch.uint8, device=dev))
+        torch.cuda.current_stream(dev).synchronize()
+        self.ptrs = [b.data_ptr() if b is not None and b.numel() else 0 for b in bufs]
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *exc):
+        if self._bufs is None:
+            for p in self.ptrs:
+                if p:
+                    self._sim.device_free(p)
+
+    def results(self):
+        out = []
+        for i, d in enumerate(self._dests):
+            if d is None:
+                continue
+            shape, t = d
+            if self._bufs is None:
+                out.append(self._sim.memcpy_dtoh(self.ptrs[i], math.prod(shape) * t.itemsize).view(t).reshape(shape))
+            elif t not in _TORCH_DESTS:
+                out.append(self._bufs[i].cpu().numpy().view(t))
+            else:
+                b = self._bufs[i]
+                out.append(b if b.shape[0] == shape[0] else b[:shape[0]])
+        return tuple(out)
+
+
+class _DeviceInput:
+    """An (N, W) float32 array at a 16-byte aligned device address (`ptr`) for the `with` block. A numpy array is copied
+    into device memory freed when the block ends (an empty one still gets an address); a CUDA tensor is used in place
+    when it is contiguous and 16-byte aligned, else copied, and torch's stream is synchronised, since the tensor may
+    still be being computed."""
+    __slots__ = ("_sim", "_keep", "ptr")
+
+    def __init__(self, sim, a):
+        self._sim = sim
+        if isinstance(a, np.ndarray):
+            self._keep, self.ptr = None, sim.device_alloc(max(a.nbytes, 16))
+            if a.nbytes:
+                try:
+                    sim.memcpy_htod(self.ptr, a)
+                except BaseException:
+                    sim.device_free(self.ptr)
+                    raise
+            return
+        import torch
+        if not a.is_contiguous() or a.data_ptr() % 16:
+            a = a.contiguous().clone()
+        torch.cuda.current_stream(a.device).synchronize()
+        self._keep, self.ptr = a, a.data_ptr()                # the tensor stays alive until the block ends
+
+    def __enter__(self):
+        return self.ptr
+
+    def __exit__(self, *exc):
+        if self._keep is None:
+            self._sim.device_free(self.ptr)
+
+
+def _depth(depth):
+    return -1 if depth is None else int(depth)
+
+
+def _is_tensor(a):
+    return not isinstance(a, np.ndarray) and hasattr(a, "data_ptr")
+
+
 def mat4_to_struct(m):
     """Row-major 4x4 math matrix -> mat4 (rows[]). The reference host stores glm::transpose(M)."""
     m = np.asarray(m, dtype=np.float32).reshape(4, 4)
@@ -461,6 +572,12 @@ class SimLOD:
     def _check(self, rc):
         if rc != 0:
             raise SimlodError(rc, self._lib.simlod_last_error().decode())
+
+    def _call(self, fn, info, *args):
+        """fn(ctx, *args, &info, &kernel_ms), raising SimlodError on failure. Returns (info, kernel ms)."""
+        ms = C.c_float(0)
+        self._check(fn(self._ctx, *args, C.byref(info), C.byref(ms)))
+        return info, ms.value
 
     def _push_uniforms(self):
         self._check(self._lib.simlod_set_uniforms(self._ctx, C.byref(self.uniforms)))
@@ -592,9 +709,7 @@ class SimLOD:
         """Save the octree, as the last completed update left it, to an octree file (simlod_save_octree): the full
         export's records and samples (np.memmap-able at the header's offsets), the nodes' counters, the box and the batch
         counters. Writes nothing into the context. Returns (ExportInfo, kernel ms)."""
-        info, ms = ExportInfo(), C.c_float(0)
-        self._check(self._lib.simlod_save_octree(self._ctx, os.fsencode(path), C.byref(info), C.byref(ms)))
-        return info, ms.value
+        return self._call(self._lib.simlod_save_octree, ExportInfo(), os.fsencode(path))
 
     def load_octree(self, path, loader_threads=16):
         """Replace the octree by an octree file's (simlod_load_octree): render it, export it or insert further batches,
@@ -611,8 +726,7 @@ class SimLOD:
         inserted points), else num_samples 16-byte samples at a 16-byte aligned device address. Returns (LasWriteInfo,
         kernel ms); on SimlodError the info is the exception's `.info` (first_invalid names an invalid sample)."""
         info, ms = LasWriteInfo(), C.c_float(0)
-        d = -1 if depth is None else int(depth)
-        rc = self._lib.simlod_write_las(self._ctx, os.fsencode(path), C.byref(params), int(samples_ptr), int(num_samples), d,
+        rc = self._lib.simlod_write_las(self._ctx, os.fsencode(path), C.byref(params), int(samples_ptr), int(num_samples), _depth(depth),
                                         C.byref(info), C.byref(ms))
         if rc != 0:
             err = SimlodError(rc, self._lib.simlod_last_error().decode())
@@ -636,16 +750,11 @@ class SimLOD:
         params = las_write_params(scale, offset, translation, writer_threads)
         if samples is None:
             return self.write_las_into(path, params, 0, 0, depth)[0]
-        if not isinstance(samples, np.ndarray) and hasattr(samples, "data_ptr"):
+        if _is_tensor(samples):
             import torch
             if not samples.is_cuda or samples.dtype != torch.float32 or samples.ndim != 2 or samples.shape[1] != 4:
                 raise ValueError("samples must be a CUDA float32 (N, 4) tensor, or a POINT_DTYPE or (N, 4) float32 array")
-            t = samples if samples.is_contiguous() and samples.data_ptr() % 16 == 0 else samples.contiguous().clone()
-            torch.cuda.current_stream(t.device).synchronize()   # the samples may still be being computed on torch's stream
-            n = t.shape[0]
-            if n and t.data_ptr():
-                return self.write_las_into(path, params, t.data_ptr(), n, depth)[0]
-            a = np.zeros((0, 4), dtype=np.float32)
+            a = samples if samples.shape[0] and samples.data_ptr() else np.zeros((0, 4), dtype=np.float32)
         else:
             a = np.asarray(samples)
             if a.dtype == POINT_DTYPE:
@@ -653,13 +762,8 @@ class SimLOD:
             if a.dtype != np.float32 or a.ndim != 2 or a.shape[1] != 4:
                 raise ValueError("samples must be a CUDA float32 (N, 4) tensor, or a POINT_DTYPE or (N, 4) float32 array")
             a = np.ascontiguousarray(a)
-        dptr = self.device_alloc(max(a.nbytes, 16))           # an empty array still needs an address: 0 is the octree
-        try:
-            if a.nbytes:
-                self.memcpy_htod(dptr, a)
-            return self.write_las_into(path, params, dptr, a.shape[0], depth)[0]
-        finally:
-            self.device_free(dptr)
+        with _DeviceInput(self, a) as ptr:                   # an empty array still gets an address: 0 is the octree
+            return self.write_las_into(path, params, ptr, a.shape[0], depth)[0]
 
     def insert_batches(self, batches):
         """Insert explicit batches (each <= 1 M points), each followed by update launches until the
@@ -727,11 +831,8 @@ class SimLOD:
     def export_octree_into(self, depth, dst_nodes, node_capacity, dst_samples, sample_capacity):
         """simlod_export_octree into caller-owned device memory (depth None or < 0: full export; all zero: size query).
         Returns (ExportInfo, kernel ms)."""
-        info, ms = ExportInfo(), C.c_float(0)
-        d = -1 if depth is None else int(depth)
-        self._check(self._lib.simlod_export_octree(self._ctx, d, int(dst_nodes), int(node_capacity), int(dst_samples),
-                                                   int(sample_capacity), C.byref(info), C.byref(ms)))
-        return info, ms.value
+        return self._call(self._lib.simlod_export_octree, ExportInfo(), _depth(depth), int(dst_nodes), int(node_capacity),
+                          int(dst_samples), int(sample_capacity))
 
     def export_octree(self, depth=None, device="cuda"):
         """The octree as flat arrays (simlod_export_octree): depth=None exports every node with its points and voxels, an
@@ -743,10 +844,8 @@ class SimLOD:
 
     def export_view_into(self, dst_nodes, node_capacity, dst_samples, sample_capacity):
         """simlod_export_view into caller-owned device memory (all zero: size query). Returns (ExportInfo, kernel ms)."""
-        info, ms = ExportInfo(), C.c_float(0)
-        self._check(self._lib.simlod_export_view(self._ctx, int(dst_nodes), int(node_capacity), int(dst_samples),
-                                                 int(sample_capacity), C.byref(info), C.byref(ms)))
-        return info, ms.value
+        return self._call(self._lib.simlod_export_view, ExportInfo(), int(dst_nodes), int(node_capacity), int(dst_samples),
+                          int(sample_capacity))
 
     def export_view(self, device="cuda"):
         """The LOD cut render() draws for the current camera and settings, as flat arrays (simlod_export_view): the drawn
@@ -759,39 +858,15 @@ class SimLOD:
         sample_capacity) -> (ExportInfo, ms)."""
         info, _ = into(0, 0, 0, 0)
         n, m = info.num_nodes, info.num_samples
-        if device == "cpu":
-            dn = self.device_alloc(n * 64)
-            ds = self.device_alloc(m * 16) if m else 0
-            try:
-                info, _ = into(dn, n, ds, m)
-                nodes = self.memcpy_dtoh(dn, n * 64).view(EXPORT_NODE_DTYPE)
-                samples = self.memcpy_dtoh(ds, m * 16).view(POINT_DTYPE)
-            finally:
-                self.device_free(dn)
-                if ds:
-                    self.device_free(ds)
-            return OctreeExport(nodes, samples, info)
-        import torch
-        dev = torch.device(device)
-        if dev.type != "cuda":
-            raise ValueError("device must be 'cpu' or a CUDA device, not %r" % device)
-        if dev.index is None:
-            dev = torch.device("cuda", self.device)
-        nodes_t = torch.empty(n * 64, dtype=torch.uint8, device=dev)
-        samples = torch.empty((m, 4), dtype=torch.float32, device=dev)
-        torch.cuda.current_stream(dev).synchronize()       # the caching allocator may hand out memory torch still uses
-        info, _ = into(nodes_t.data_ptr(), n, samples.data_ptr() if m else 0, m)
-        nodes = nodes_t.cpu().numpy().view(EXPORT_NODE_DTYPE)
-        return OctreeExport(nodes, samples, info)
+        with _Results(self, device, (((n,), EXPORT_NODE_DTYPE), ((m,), POINT_DTYPE))) as r:
+            info, _ = into(r.ptrs[0], n, r.ptrs[1], m)
+            return OctreeExport(*r.results(), info)
 
     def query_region_into(self, region, depth, dst_samples, sample_capacity):
         """simlod_query_region into caller-owned device memory (depth None or < 0: the inserted points; dst_samples 0:
         size query). Returns (SimlodQueryInfo, kernel ms)."""
-        info, ms = SimlodQueryInfo(), C.c_float(0)
-        d = -1 if depth is None else int(depth)
-        self._check(self._lib.simlod_query_region(self._ctx, C.byref(region), d, int(dst_samples), int(sample_capacity),
-                                                  C.byref(info), C.byref(ms)))
-        return info, ms.value
+        return self._call(self._lib.simlod_query_region, SimlodQueryInfo(), C.byref(region), _depth(depth), int(dst_samples),
+                          int(sample_capacity))
 
     def query_region(self, region, depth=None, device="cuda"):
         """The samples inside `region` (Region.box / sphere / planes), filtered on the GPU (simlod_query_region): with
@@ -802,32 +877,15 @@ class SimLOD:
         device="cpu" a numpy POINT_DTYPE array."""
         info, _ = self.query_region_into(region, depth, 0, 0)
         m = info.num_samples
-        if device == "cpu":
-            ds = self.device_alloc(m * 16) if m else 0
-            try:
-                if m:
-                    info, _ = self.query_region_into(region, depth, ds, m)
-                return self.memcpy_dtoh(ds, m * 16).view(POINT_DTYPE), info
-            finally:
-                if ds:
-                    self.device_free(ds)
-        import torch
-        dev = torch.device(device)
-        if dev.type != "cuda":
-            raise ValueError("device must be 'cpu' or a CUDA device, not %r" % device)
-        if dev.index is None:
-            dev = torch.device("cuda", self.device)
-        samples = torch.empty((m, 4), dtype=torch.float32, device=dev)
-        torch.cuda.current_stream(dev).synchronize()       # the caching allocator may hand out memory torch still uses
-        if m:
-            info, _ = self.query_region_into(region, depth, samples.data_ptr(), m)
-        return samples, info
+        with _Results(self, device, (((m,), POINT_DTYPE),)) as r:
+            if m:
+                info, _ = self.query_region_into(region, depth, r.ptrs[0], m)
+            return r.results()[0], info
 
     def pick_into(self, pixels, dst_index, dst_samples):
         """simlod_pick into caller-owned device memory: pixels None for the whole frame, else an (N, 2) array of (x, y);
         dst_index (int64) and dst_samples (16-byte samples, 0 for none) both 0: info only. Returns (SimlodPickInfo,
         kernel ms)."""
-        info, ms = SimlodPickInfo(), C.c_float(0)
         if pixels is None:
             ptr, n = None, 0
         else:
@@ -840,8 +898,7 @@ class SimLOD:
             n = a.shape[0]
             keep = a if n else np.zeros(2, dtype=np.uint32)        # an empty list is still a list (and is refused)
             ptr = keep.ctypes.data_as(C.POINTER(C.c_uint32))
-        self._check(self._lib.simlod_pick(self._ctx, ptr, n, int(dst_index), int(dst_samples), C.byref(info), C.byref(ms)))
-        return info, ms.value
+        return self._call(self._lib.simlod_pick, SimlodPickInfo(), ptr, n, int(dst_index), int(dst_samples))
 
     def pick(self, pixels=None, device="cuda", samples=False):
         """The sample under each pixel of the frame render() draws for the current uniforms (simlod_pick): an index into
@@ -851,41 +908,17 @@ class SimLOD:
         colour bits), zeros where the index is -1. device="cuda": torch tensors in device memory; device="cpu": numpy
         arrays (the samples as POINT_DTYPE). Returns (index, info) or, with samples=True, (index, samples, info)."""
         shape = (self.height, self.width) if pixels is None else (len(np.asarray(pixels)),)
-        n = int(np.prod(shape))
-        if device == "cpu":
-            di = self.device_alloc(max(n, 1) * 8)
-            ds = self.device_alloc(max(n, 1) * 16) if samples else 0
-            try:
-                info, _ = self.pick_into(pixels, di, ds)
-                index = self.memcpy_dtoh(di, n * 8).view(np.int64).reshape(shape)
-                picked = self.memcpy_dtoh(ds, n * 16).view(POINT_DTYPE).reshape(shape) if samples else None
-            finally:
-                self.device_free(di)
-                if ds:
-                    self.device_free(ds)
-            return (index, picked, info) if samples else (index, info)
-        import torch
-        dev = torch.device(device)
-        if dev.type != "cuda":
-            raise ValueError("device must be 'cpu' or a CUDA device, not %r" % device)
-        if dev.index is None:
-            dev = torch.device("cuda", self.device)
-        index = torch.empty(shape, dtype=torch.int64, device=dev)
-        picked = torch.empty(shape + (4,), dtype=torch.float32, device=dev) if samples else None
-        torch.cuda.current_stream(dev).synchronize()       # the caching allocator may hand out memory torch still uses
-        info, _ = self.pick_into(pixels, index.data_ptr() if n else 0, picked.data_ptr() if samples and n else 0)
-        return (index, picked, info) if samples else (index, info)
+        with _Results(self, device, ((shape, I8), (shape, POINT_DTYPE) if samples else None)) as r:
+            info, _ = self.pick_into(pixels, *r.ptrs)
+            return r.results() + (info,)
 
     def query_nearest_into(self, queries_ptr, n, k, depth, max_radius, dst_index, dst_dist2, dst_samples):
         """simlod_query_nearest on caller-owned device memory: n 16-byte query records at queries_ptr, destinations
         [n][k] int64 / float32 / 16-byte samples, each 0 for not written (depth None or < 0: the inserted points;
         max_radius None: no limit). Returns (SimlodNearestInfo, kernel ms)."""
-        info, ms = SimlodNearestInfo(), C.c_float(0)
-        d = -1 if depth is None else int(depth)
         r = float("inf") if max_radius is None else float(max_radius)
-        self._check(self._lib.simlod_query_nearest(self._ctx, int(queries_ptr), int(n), int(k), d, r, int(dst_index),
-                                                   int(dst_dist2), int(dst_samples), C.byref(info), C.byref(ms)))
-        return info, ms.value
+        return self._call(self._lib.simlod_query_nearest, SimlodNearestInfo(), int(queries_ptr), int(n), int(k), _depth(depth), r,
+                          int(dst_index), int(dst_dist2), int(dst_samples))
 
     def query_nearest(self, queries, k=8, depth=None, max_radius=None, device="cuda", samples=False):
         """The k nearest samples of each query position (simlod_query_nearest), exact: with depth=None among the
@@ -907,70 +940,34 @@ class SimLOD:
         passed as it is; anything else is copied, into memory freed when the block ends."""
         if isinstance(queries, np.ndarray) and queries.dtype == POINT_DTYPE:
             queries = queries.view(np.float32).reshape(-1, 4)
-        if not isinstance(queries, np.ndarray) and hasattr(queries, "data_ptr"):
+        if _is_tensor(queries):
             import torch
             if not queries.is_cuda or queries.ndim != 2 or queries.shape[1] not in (3, 4):
                 raise ValueError("queries must be an (N, 3) or (N, 4) CUDA tensor or numpy array")
             q = queries.detach().to(torch.float32)
-            if q.shape[1] == 3 or not q.is_contiguous() or q.data_ptr() % 16:
-                q4 = torch.zeros((q.shape[0], 4), dtype=torch.float32, device=q.device)
-                q4[:, :3] = q[:, :3]
-                q = q4
-            torch.cuda.current_stream(q.device).synchronize()  # the queries may still be being computed on torch's stream
-            yield q.data_ptr(), q.shape[0]                      # q stays alive until the block ends
-            return
-        a = np.asarray(queries)
-        if a.ndim != 2 or a.shape[1] not in (3, 4):
-            raise ValueError("queries must be an (N, 3) or (N, 4) CUDA tensor or numpy array")
-        q = np.zeros((a.shape[0], 4), dtype=np.float32)
-        q[:, :3] = a[:, :3]
-        dq = self.device_alloc(max(q.nbytes, 16))
-        try:
-            self.memcpy_htod(dq, q)
-            yield dq, q.shape[0]
-        finally:
-            self.device_free(dq)
+            if q.shape[1] == 3:
+                q = torch.cat([q, q.new_zeros((q.shape[0], 1))], dim=1)
+        else:
+            a = np.asarray(queries)
+            if a.ndim != 2 or a.shape[1] not in (3, 4):
+                raise ValueError("queries must be an (N, 3) or (N, 4) CUDA tensor or numpy array")
+            q = np.zeros((a.shape[0], 4), dtype=np.float32)
+            q[:, :3] = a[:, :3]
+        with _DeviceInput(self, q) as ptr:
+            yield ptr, q.shape[0]
 
     def _nearest(self, qptr, n, k, depth, max_radius, device, samples):
-        if device == "cpu":
-            m = max(n * k, 1)
-            di, dd = self.device_alloc(m * 8), self.device_alloc(m * 4)
-            ds = self.device_alloc(m * 16) if samples else 0
-            try:
-                info, _ = self.query_nearest_into(qptr, n, k, depth, max_radius, di, dd, ds)
-                index = self.memcpy_dtoh(di, n * k * 8).view(np.int64).reshape(n, k)
-                dist2 = self.memcpy_dtoh(dd, n * k * 4).view(np.float32).reshape(n, k)
-                found = self.memcpy_dtoh(ds, n * k * 16).view(POINT_DTYPE).reshape(n, k) if samples else None
-            finally:
-                for p in (di, dd, ds):
-                    if p:
-                        self.device_free(p)
-            return (index, dist2, found, info) if samples else (index, dist2, info)
-        import torch
-        dev = torch.device(device)
-        if dev.type != "cuda":
-            raise ValueError("device must be 'cpu' or a CUDA device, not %r" % device)
-        if dev.index is None:
-            dev = torch.device("cuda", self.device)
-        index = torch.empty((n, k), dtype=torch.int64, device=dev)
-        dist2 = torch.empty((n, k), dtype=torch.float32, device=dev)
-        found = torch.empty((n, k, 4), dtype=torch.float32, device=dev) if samples else None
-        torch.cuda.current_stream(dev).synchronize()       # the caching allocator may hand out memory torch still uses
-        info, _ = self.query_nearest_into(qptr, n, k, depth, max_radius, index.data_ptr() if n else 0,
-                                          dist2.data_ptr() if n else 0, found.data_ptr() if samples and n else 0)
-        return (index, dist2, found, info) if samples else (index, dist2, info)
+        with _Results(self, device, (((n, k), I8), ((n, k), F4), ((n, k), POINT_DTYPE) if samples else None)) as r:
+            info, _ = self.query_nearest_into(qptr, n, k, depth, max_radius, *r.ptrs)
+            return r.results() + (info,)
 
     def query_radius_into(self, queries_ptr, n, radius, depth, dst_offsets, dst_index, dst_dist2, dst_samples, capacity):
         """simlod_query_radius on caller-owned device memory: n 16-byte query records at queries_ptr; dst_offsets int64
         [n + 1]; dst_index / dst_dist2 / dst_samples int64 / float32 / 16-byte samples with `capacity` neighbour slots
         each, 0 for not written (all three 0: size query, which fills the offsets when dst_offsets is not 0; depth None or
         < 0: the inserted points). Returns (SimlodRadiusInfo, kernel ms)."""
-        info, ms = SimlodRadiusInfo(), C.c_float(0)
-        d = -1 if depth is None else int(depth)
-        self._check(self._lib.simlod_query_radius(self._ctx, int(queries_ptr), int(n), float(radius), d, int(dst_offsets),
-                                                  int(dst_index), int(dst_dist2), int(dst_samples), int(capacity),
-                                                  C.byref(info), C.byref(ms)))
-        return info, ms.value
+        return self._call(self._lib.simlod_query_radius, SimlodRadiusInfo(), int(queries_ptr), int(n), float(radius), _depth(depth),
+                          int(dst_offsets), int(dst_index), int(dst_dist2), int(dst_samples), int(capacity))
 
     def query_radius(self, queries, radius, depth=None, device="cuda", samples=False):
         """Every sample within `radius` of each query position (simlod_query_radius), exact: with depth=None among the
@@ -986,47 +983,16 @@ class SimLOD:
         with self._device_queries(queries) as (qptr, n):
             info, _ = self.query_radius_into(qptr, n, radius, depth, 0, 0, 0, 0, 0)
             m = info.num_found
-            if device == "cpu":
-                do = self.device_alloc((n + 1) * 8)
-                di, dd = self.device_alloc(max(m, 1) * 8), self.device_alloc(max(m, 1) * 4)
-                ds = self.device_alloc(max(m, 1) * 16) if samples else 0
-                try:
-                    info, _ = self.query_radius_into(qptr, n, radius, depth, do, di, dd, ds, m)
-                    offsets = self.memcpy_dtoh(do, (n + 1) * 8).view(np.int64)
-                    index = self.memcpy_dtoh(di, m * 8).view(np.int64)
-                    dist2 = self.memcpy_dtoh(dd, m * 4).view(np.float32)
-                    found = self.memcpy_dtoh(ds, m * 16).view(POINT_DTYPE) if samples else None
-                finally:
-                    for p in (do, di, dd, ds):
-                        if p:
-                            self.device_free(p)
-                return (offsets, index, dist2, found, info) if samples else (offsets, index, dist2, info)
-            import torch
-            dev = torch.device(device)
-            if dev.type != "cuda":
-                raise ValueError("device must be 'cpu' or a CUDA device, not %r" % device)
-            if dev.index is None:
-                dev = torch.device("cuda", self.device)
-            offsets = torch.empty(n + 1, dtype=torch.int64, device=dev)
-            index = torch.empty(max(m, 1), dtype=torch.int64, device=dev)
-            dist2 = torch.empty(max(m, 1), dtype=torch.float32, device=dev)
-            found = torch.empty((max(m, 1), 4), dtype=torch.float32, device=dev) if samples else None
-            torch.cuda.current_stream(dev).synchronize()       # the caching allocator may hand out memory torch still uses
-            info, _ = self.query_radius_into(qptr, n, radius, depth, offsets.data_ptr(), index.data_ptr(), dist2.data_ptr(),
-                                             found.data_ptr() if samples else 0, m)
-            index, dist2 = index[:m], dist2[:m]
-            found = found[:m] if samples else None
-            return (offsets, index, dist2, found, info) if samples else (offsets, index, dist2, info)
+            with _Results(self, device, (((n + 1,), I8), ((m,), I8), ((m,), F4), ((m,), POINT_DTYPE) if samples else None), keep=True) as r:
+                info, _ = self.query_radius_into(qptr, n, radius, depth, *r.ptrs, m)
+                return r.results() + (info,)
 
     def query_ray_into(self, rays_ptr, n, radius, depth, dst_index, dst_t, dst_h2, dst_samples):
         """simlod_query_ray on caller-owned device memory: n 32-byte ray records (ox, oy, oz, tmin, dx, dy, dz, tmax) at
         rays_ptr, destinations [n] int64 / float32 / float32 / 16-byte samples, each 0 for not written (depth None or < 0:
         the inserted points). Returns (SimlodRayInfo, kernel ms)."""
-        info, ms = SimlodRayInfo(), C.c_float(0)
-        d = -1 if depth is None else int(depth)
-        self._check(self._lib.simlod_query_ray(self._ctx, int(rays_ptr), int(n), float(radius), d, int(dst_index), int(dst_t),
-                                               int(dst_h2), int(dst_samples), C.byref(info), C.byref(ms)))
-        return info, ms.value
+        return self._call(self._lib.simlod_query_ray, SimlodRayInfo(), int(rays_ptr), int(n), float(radius), _depth(depth),
+                          int(dst_index), int(dst_t), int(dst_h2), int(dst_samples))
 
     def query_ray(self, origins, directions, radius, tmin=0.0, tmax=None, depth=None, device="cuda", samples=False):
         """The first stored sample along each ray (simlod_query_ray), exact: among the samples within `radius` of the ray
@@ -1039,8 +1005,7 @@ class SimLOD:
         export_octree(depth).samples, -1 for no hit; (N,) float32 t, +inf for no hit; (N,) float32 squared distances
         from the ray, +inf for no hit; (N, 4) float32 samples in the export's layout, zeros for no hit. device="cuda":
         torch tensors in device memory; device="cpu": numpy arrays (the samples as POINT_DTYPE)."""
-        on_device = not isinstance(origins, np.ndarray) and hasattr(origins, "data_ptr")
-        if on_device:
+        if _is_tensor(origins):
             import torch
             o = origins.detach()
             d = directions.detach() if hasattr(directions, "data_ptr") else torch.as_tensor(np.asarray(directions), device=o.device)
@@ -1054,53 +1019,18 @@ class SimLOD:
                 v = default if v is None else v
                 r[:, col] = v.to(device=o.device, dtype=torch.float32) if hasattr(v, "data_ptr") else \
                     torch.as_tensor(np.broadcast_to(np.asarray(v, dtype=np.float32), (n,)).copy(), device=o.device)
-            torch.cuda.current_stream(o.device).synchronize()  # the rays may still be being computed on torch's stream
-            return self._ray(r.data_ptr(), n, radius, depth, device, samples)
-        o, d = np.asarray(origins), np.asarray(directions)
-        if o.ndim != 2 or o.shape[1] != 3 or d.shape != o.shape:
-            raise ValueError("origins and directions must be (N, 3) CUDA tensors or numpy arrays of one shape")
-        n = o.shape[0]
-        r = np.empty((n, 8), dtype=np.float32)
-        r[:, 0:3], r[:, 4:7] = o, d
-        r[:, 3] = np.broadcast_to(np.asarray(0.0 if tmin is None else tmin, dtype=np.float32), (n,))
-        r[:, 7] = np.broadcast_to(np.asarray(np.inf if tmax is None else tmax, dtype=np.float32), (n,))
-        dr = self.device_alloc(max(r.nbytes, 32))
-        try:
-            self.memcpy_htod(dr, r)
-            return self._ray(dr, n, radius, depth, device, samples)
-        finally:
-            self.device_free(dr)
-
-    def _ray(self, rptr, n, radius, depth, device, samples):
-        if device == "cpu":
-            m = max(n, 1)
-            di, dt, dh = self.device_alloc(m * 8), self.device_alloc(m * 4), self.device_alloc(m * 4)
-            ds = self.device_alloc(m * 16) if samples else 0
-            try:
-                info, _ = self.query_ray_into(rptr, n, radius, depth, di, dt, dh, ds)
-                index = self.memcpy_dtoh(di, n * 8).view(np.int64)
-                t = self.memcpy_dtoh(dt, n * 4).view(np.float32)
-                h2 = self.memcpy_dtoh(dh, n * 4).view(np.float32)
-                found = self.memcpy_dtoh(ds, n * 16).view(POINT_DTYPE) if samples else None
-            finally:
-                for p in (di, dt, dh, ds):
-                    if p:
-                        self.device_free(p)
-            return (index, t, h2, found, info) if samples else (index, t, h2, info)
-        import torch
-        dev = torch.device(device)
-        if dev.type != "cuda":
-            raise ValueError("device must be 'cpu' or a CUDA device, not %r" % device)
-        if dev.index is None:
-            dev = torch.device("cuda", self.device)
-        index = torch.empty(n, dtype=torch.int64, device=dev)
-        t = torch.empty(n, dtype=torch.float32, device=dev)
-        h2 = torch.empty(n, dtype=torch.float32, device=dev)
-        found = torch.empty((n, 4), dtype=torch.float32, device=dev) if samples else None
-        torch.cuda.current_stream(dev).synchronize()       # the caching allocator may hand out memory torch still uses
-        info, _ = self.query_ray_into(rptr, n, radius, depth, index.data_ptr() if n else 0, t.data_ptr() if n else 0,
-                                      h2.data_ptr() if n else 0, found.data_ptr() if samples and n else 0)
-        return (index, t, h2, found, info) if samples else (index, t, h2, info)
+        else:
+            o, d = np.asarray(origins), np.asarray(directions)
+            if o.ndim != 2 or o.shape[1] != 3 or d.shape != o.shape:
+                raise ValueError("origins and directions must be (N, 3) CUDA tensors or numpy arrays of one shape")
+            n = o.shape[0]
+            r = np.empty((n, 8), dtype=np.float32)
+            r[:, 0:3], r[:, 4:7] = o, d
+            r[:, 3] = np.broadcast_to(np.asarray(0.0 if tmin is None else tmin, dtype=np.float32), (n,))
+            r[:, 7] = np.broadcast_to(np.asarray(np.inf if tmax is None else tmax, dtype=np.float32), (n,))
+        with _DeviceInput(self, r) as rptr, _Results(self, device, (((n,), I8), ((n,), F4), ((n,), F4), ((n,), POINT_DTYPE) if samples else None)) as out:
+            info, _ = self.query_ray_into(rptr, n, radius, depth, *out.ptrs)
+            return out.results() + (info,)
 
     def host_alloc(self, nbytes):
         p = C.c_void_p()

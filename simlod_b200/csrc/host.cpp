@@ -210,13 +210,9 @@ struct SimlodContext {
     CUevent evStaged[MAX_STAGING_SLOTS] = {}, evStagingFree[MAX_STAGING_SLOTS] = {};
     CUdeviceptr exportScratch = 0;     // octree export and region query: see scratchFor()
     uint64_t exportScratchBytes = 0;
-    void* hExportCtl = nullptr;        // pinned copy of ExportCtl / QueryCtl / NearestCtl / RayCtl (CTL_HOST_BYTES)
-    CUdeviceptr pickScratch = 0;       // pick: key frame | index frame | hit counter | pixel list
-    uint64_t pickScratchBytes = 0;
-    CUdeviceptr nearestScratch = 0;    // k nearest: per query home | slot | bucket, per home count | offset | run start, NearestCtl
-    uint64_t nearestScratchBytes = 0;
-    CUdeviceptr rayCtl = 0;            // rays: RayCtl
-    uint64_t rayCtlBytes = 0;
+    void* hExportCtl = nullptr;        // pinned copy of the control structs read back (StageClock::finish)
+    CUdeviceptr queryScratch = 0;      // the plan's consumers, one at a time: pick's frames, the buckets and passes of k
+    uint64_t queryScratchBytes = 0;    // nearest and radius, RayCtl
     CUdeviceptr fileWindow = 0;        // octree files: FILE_WINDOW_BYTES of samples staged on the device
     CUdeviceptr fileTables = 0;        // octree load: records | plan | error word, sized for nodes[]
     CUdeviceptr lasWindow = 0;         // LAS writer: one window of records, then LasWriteCtl
@@ -634,9 +630,7 @@ void simlod_destroy(SimlodContext* ctx) {
         }
         if (ctx->exportScratch) D(cuMemFree)(ctx->exportScratch);
         if (ctx->hExportCtl) D(cuMemFreeHost)(ctx->hExportCtl);
-        if (ctx->pickScratch) D(cuMemFree)(ctx->pickScratch);
-        if (ctx->nearestScratch) D(cuMemFree)(ctx->nearestScratch);
-        if (ctx->rayCtl) D(cuMemFree)(ctx->rayCtl);
+        if (ctx->queryScratch) D(cuMemFree)(ctx->queryScratch);
         if (ctx->fileWindow) D(cuMemFree)(ctx->fileWindow);
         if (ctx->fileTables) D(cuMemFree)(ctx->fileTables);
         if (ctx->lasWindow) D(cuMemFree)(ctx->lasWindow);
@@ -1470,6 +1464,52 @@ constexpr size_t CTL_HOST_BYTES = 128;      // the pinned copy of the control wo
 static_assert(sizeof(ExportCtl) <= CTL_HOST_BYTES && sizeof(QueryCtl) <= CTL_HOST_BYTES && sizeof(NearestCtl) <= CTL_HOST_BYTES &&
               sizeof(RayCtl) <= CTL_HOST_BYTES && sizeof(NearestCtl) + sizeof(RadiusCtl) <= CTL_HOST_BYTES, "pinned control word");
 
+// Consecutive 16-byte aligned regions of one allocation: take() returns the offset of the next one
+struct Layout { uint64_t bytes = 0; uint64_t take(uint64_t n) { const uint64_t off = bytes; bytes += align16(n); return off; } };
+
+// A control struct on the device and the host copy it is read into
+struct CtlRead { CUdeviceptr src; void* dst; size_t bytes; };
+
+// Up to four ordered marks on streamMain, on the context's four events; stage i is the time from mark i to mark i + 1.
+// finish() makes the last mark, waits for it and reads the stages into ms[]. Control structs to read back are copied one
+// after the other into the pinned control word behind the mark, and the wait is the one synchronisation of streamMain
+// that brings them to their host copies; without them it waits on the mark's event.
+struct StageClock {
+    SimlodContext* ctx; CUevent ev[4]; int marks = 0;
+    explicit StageClock(SimlodContext* c) : ctx(c), ev{c->evStart, c->evEnd, c->evTotalStart, c->evTotalEnd} {}
+    int mark() {                            // the pinned control word is allocated before any stage is timed
+        if (marks == 4) return fail(SIMLOD_ERR_INVALID, "internal: a stage clock has four marks");
+        if (!ctx->hExportCtl) CU(D(cuMemHostAlloc)(&ctx->hExportCtl, CTL_HOST_BYTES, 0));
+        CU(D(cuEventRecord)(ev[marks++], ctx->streamMain)); return SIMLOD_OK;
+    }
+    int finish(float* ms, std::initializer_list<CtlRead> reads = {}) {
+        int rc = mark(); if (rc) return rc;
+        uint8_t* const h = (uint8_t*)ctx->hExportCtl;
+        size_t at = 0;
+        for (const CtlRead& r : reads) { CU(D(cuMemcpyDtoHAsync)(h + at, r.src, r.bytes, ctx->streamMain)); at += r.bytes; }
+        if (reads.size()) CU(D(cuStreamSynchronize)(ctx->streamMain)); else CU(D(cuEventSynchronize)(ev[marks - 1]));
+        at = 0;
+        for (const CtlRead& r : reads) { memcpy(r.dst, h + at, r.bytes); at += r.bytes; }
+        for (int i = 0; i + 1 < marks; i++) CU(D(cuEventElapsedTime)(&ms[i], ev[i], ev[i + 1]));
+        return SIMLOD_OK;
+    }
+};
+
+// the refusal of a depth deeper than the octree's deepest level, for the entry point `what`
+int checkDepth(const char* what, int32_t depth) {
+    return depth > SIMLOD_MAX_DEPTH ? fail(SIMLOD_ERR_INVALID, "%s depth %d exceeds the octree's maximum depth %d", what, depth, (int)SIMLOD_MAX_DEPTH) : SIMLOD_OK;
+}
+
+// the refusal of the first address that is not a multiple of its alignment (or null, where one is required), for the
+// entry point `what`
+struct Aligned { const char* name; uint64_t addr; uint64_t align; bool required = false; };
+int checkAligned(const char* what, std::initializer_list<Aligned> addrs) {
+    for (const Aligned& a : addrs)
+        if (a.addr % a.align || (a.required && !a.addr))
+            return fail(SIMLOD_ERR_INVALID, "%s: %s must be %s%llu-byte aligned", what, a.name, a.required ? "a device address, " : "", (unsigned long long)a.align);
+    return SIMLOD_OK;
+}
+
 // The context's export / query scratch, sized by its buffers: one record, node index and first item per node of nodes[],
 // and one chunk item per chunk the heap can hold. The view adds per node a drawn byte, and per record a mark byte, an
 // index and a second record and node index; the query adds one word per item. The control word comes last.
@@ -1484,18 +1524,16 @@ int scratchFor(SimlodContext* ctx, ScratchUse use, Scratch* s) {
     const uint64_t n = (uint64_t)(uint32_t)(ctx->buf.nodes_bytes / sizeof(SimlodNode));
     s->maxRecords = (uint32_t)n;
     s->itemsCap = ctx->buf.persistent_bytes / SIMLOD_CHUNK_STRIDE + 1;
-    uint64_t at = 0;
-    auto take = [&](uint64_t bytes) { const uint64_t off = at; at += align16(bytes); return off; };
-    const uint64_t rec = take(n * sizeof(SimlodExportNode)), recNode = take(n * 4), recItem = take(n * 8), items = take(s->itemsCap * 16);
+    Layout l;
+    const uint64_t rec = l.take(n * sizeof(SimlodExportNode)), recNode = l.take(n * 4), recItem = l.take(n * 8), items = l.take(s->itemsCap * 16);
     uint64_t drawn = 0, viewRec = 0, viewNode = 0, mark = 0, index = 0, words = 0;
     if (use == ScratchUse::VIEW) {
-        drawn = take(n); mark = take(n); index = take(n * 4);
-        viewRec = take(n * sizeof(SimlodExportNode)); viewNode = take(n * 4);
+        drawn = l.take(n); mark = l.take(n); index = l.take(n * 4);
+        viewRec = l.take(n * sizeof(SimlodExportNode)); viewNode = l.take(n * 4);
     }
-    if (use == ScratchUse::QUERY) words = take(s->itemsCap * 8);
-    const uint64_t ctl = take(use == ScratchUse::QUERY ? sizeof(QueryCtl) : sizeof(ExportCtl));
-    int rc = growDevice(&ctx->exportScratch, &ctx->exportScratchBytes, at); if (rc) return rc;
-    if (!ctx->hExportCtl) CU(D(cuMemHostAlloc)(&ctx->hExportCtl, CTL_HOST_BYTES, 0));
+    if (use == ScratchUse::QUERY) words = l.take(s->itemsCap * 8);
+    const uint64_t ctl = l.take(use == ScratchUse::QUERY ? sizeof(QueryCtl) : sizeof(ExportCtl));
+    int rc = growDevice(&ctx->exportScratch, &ctx->exportScratchBytes, l.bytes); if (rc) return rc;
     const CUdeviceptr base = ctx->exportScratch;
     s->rec = base + rec; s->recNode = base + recNode; s->recItem = base + recItem; s->items = base + items; s->ctl = base + ctl;
     s->words = use == ScratchUse::QUERY ? base + words : 0;
@@ -1525,12 +1563,13 @@ struct ExportPlanned {
     ExportCtl c{};
     float ms = 0.0f;
 };
-int exportPlan(SimlodContext* ctx, int32_t depth, const SimlodUniforms* view, ExportPlanned* p) {
+int exportPlan(SimlodContext* ctx, int32_t depth, const SimlodUniforms* view, ExportPlanned* p, float* kernel_ms = nullptr) {
+    struct Report { float* dst; const float& ms; ~Report() { if (dst) *dst = ms; } } report{kernel_ms, p->ms};   // on every return
     Scratch& s = p->s;
     int rc = scratchFor(ctx, view ? ScratchUse::VIEW : ScratchUse::EXPORT, &s); if (rc) return rc;
     CUdeviceptr nodes = ctx->buf.nodes, stats = ctx->buf.stats;
     // stage 1: the view's drawn flags (one thread per node), plan (one block) and the chunk-list walk, all into scratch only
-    CU(D(cuEventRecord)(ctx->evStart, ctx->streamMain));
+    StageClock clock(ctx); rc = clock.mark(); if (rc) return rc;
     if (view) {
         SimlodUniforms u = *view;
         rc = launch(ctx, ctx->fn[K_EXPORT_VIEW_FLAGS], (unsigned)ctx->numSMs * 4, 256, ctx->streamMain, nodes, stats, u, s.maxRecords, s.view.drawn);
@@ -1541,13 +1580,18 @@ int exportPlan(SimlodContext* ctx, int32_t depth, const SimlodUniforms* view, Ex
     }
     if (rc) return rc;
     rc = launchCollect(ctx, s); if (rc) return rc;
-    CU(D(cuEventRecord)(ctx->evEnd, ctx->streamMain));
-    CU(D(cuMemcpyDtoHAsync)(ctx->hExportCtl, s.ctl, sizeof(ExportCtl), ctx->streamMain));
-    CU(D(cuStreamSynchronize)(ctx->streamMain));
-    p->c = *(const ExportCtl*)ctx->hExportCtl;
-    CU(D(cuEventElapsedTime)(&p->ms, ctx->evStart, ctx->evEnd));
+    rc = clock.finish(&p->ms, {{s.ctl, &p->c, sizeof p->c}}); if (rc) return rc;
     if (p->c.error) return failInconsistent(p->c.error);
     return SIMLOD_OK;
+}
+
+// The fields NearestArgs, RadiusArgs and RayArgs share: the plan's records and chunk items, the cut and the octree cube
+extern "C++" template <class Args> Args planArgs(const ExportPlanned& p, const SimlodUniforms& u, int32_t depth) {
+    Args a{};
+    a.rec = devPtr(p.s.rec); a.recItem = devPtr(p.s.recItem); a.items = devPtr(p.s.items);
+    a.numRecords = p.c.numNodes; a.depth = depth < 0 ? -1 : depth;
+    std::copy_n(u.boxMin, 3, a.boxMin); std::copy_n(u.boxMax, 3, a.boxMax);
+    return a;
 }
 
 // The export of simlod_export_octree (view == nullptr) and simlod_export_view (the LOD cut for *view).
@@ -1555,12 +1599,10 @@ int exportOctree(SimlodContext* ctx, int32_t depth, const SimlodUniforms* view, 
                  uint64_t dst_samples, uint64_t sample_capacity, SimlodExportInfo* info, float* kernel_ms) {
     int rc = setCurrent(ctx); if (rc) return rc;
     if (!info) return fail(SIMLOD_ERR_INVALID, "null info");
-    if (depth > SIMLOD_MAX_DEPTH) return fail(SIMLOD_ERR_INVALID, "export depth %d exceeds the octree's maximum depth %d", depth, (int)SIMLOD_MAX_DEPTH);
-    if (dst_nodes % 16 || dst_samples % 16) return fail(SIMLOD_ERR_INVALID, "export destinations must be 16-byte aligned");
+    rc = checkDepth("export", depth); if (rc) return rc;
+    rc = checkAligned("export", {{"dst_nodes", dst_nodes, 16}, {"dst_samples", dst_samples, 16}}); if (rc) return rc;
     ExportPlanned p;
-    rc = exportPlan(ctx, depth, view, &p);
-    if (kernel_ms) *kernel_ms = p.ms;
-    if (rc) return rc;
+    rc = exportPlan(ctx, depth, view, &p, kernel_ms); if (rc) return rc;
     const ExportCtl c = p.c;
     info->num_nodes = c.numNodes; info->max_level = c.maxLevel;
     info->num_samples = c.numSamples; info->num_points = c.numPoints; info->num_voxels = c.numVoxels;
@@ -1571,13 +1613,11 @@ int exportOctree(SimlodContext* ctx, int32_t depth, const SimlodUniforms* view, 
         return fail(SIMLOD_ERR_INVALID, "sample destination holds %llu samples, the export has %llu", (unsigned long long)(dst_samples ? sample_capacity : 0), (unsigned long long)c.numSamples);
     // stage 2: gather into the destination
     CUdeviceptr dn = (CUdeviceptr)dst_nodes, ds = (CUdeviceptr)dst_samples;
-    CU(D(cuEventRecord)(ctx->evTotalStart, ctx->streamMain));
+    StageClock clock(ctx); rc = clock.mark(); if (rc) return rc;
     rc = launch(ctx, ctx->fn[K_EXPORT_GATHER], (unsigned)ctx->numSMs * 4, 256, ctx->streamMain, p.s.rec, dn, p.s.items, ds, p.s.ctl);
     if (rc) return rc;
-    CU(D(cuEventRecord)(ctx->evTotalEnd, ctx->streamMain));
-    CU(D(cuEventSynchronize)(ctx->evTotalEnd));
     float gatherMs = 0.0f;
-    CU(D(cuEventElapsedTime)(&gatherMs, ctx->evTotalStart, ctx->evTotalEnd));
+    rc = clock.finish(&gatherMs); if (rc) return rc;
     if (kernel_ms) *kernel_ms = p.ms + gatherMs;
     return SIMLOD_OK;
 }
@@ -1623,29 +1663,26 @@ int simlod_query_region(SimlodContext* ctx, const SimlodRegion* region, int32_t 
                         uint64_t sample_capacity, SimlodQueryInfo* info, float* kernel_ms) {
     int rc = setCurrent(ctx); if (rc) return rc;
     if (!info) return fail(SIMLOD_ERR_INVALID, "null info");
-    if (depth > SIMLOD_MAX_DEPTH) return fail(SIMLOD_ERR_INVALID, "query depth %d exceeds the octree's maximum depth %d", depth, (int)SIMLOD_MAX_DEPTH);
-    if (dst_samples % 16) return fail(SIMLOD_ERR_INVALID, "query destination must be 16-byte aligned");
+    rc = checkDepth("query", depth); if (rc) return rc;
+    rc = checkAligned("query", {{"dst_samples", dst_samples, 16}}); if (rc) return rc;
     rc = checkRegion(region); if (rc) return rc;
     Scratch sc;
     rc = scratchFor(ctx, ScratchUse::QUERY, &sc); if (rc) return rc;
     CUdeviceptr nodes = ctx->buf.nodes, stats = ctx->buf.stats;
     SimlodRegion rg = *region;
     QueryBox box;
-    for (int a = 0; a < 3; a++) { box.mn[a] = ctx->uniforms.boxMin[a]; box.mx[a] = ctx->uniforms.boxMax[a]; }
+    std::copy_n(ctx->uniforms.boxMin, 3, box.mn); std::copy_n(ctx->uniforms.boxMax, 3, box.mx);
     // stage 1, into scratch only: plan (one block), the chunk-list walk, the per-item counts and their scan
-    CU(D(cuEventRecord)(ctx->evStart, ctx->streamMain));
+    StageClock clock(ctx); rc = clock.mark(); if (rc) return rc;
     rc = launch(ctx, ctx->fn[K_QUERY_PLAN], 1, 1024, ctx->streamMain, nodes, stats, depth, sc.maxRecords, sc.rec, sc.recNode, sc.recItem, sc.ctl, rg, box);
     if (rc) return rc;
     rc = launchCollect(ctx, sc); if (rc) return rc;
     rc = launch(ctx, ctx->fn[K_QUERY_COUNT], (unsigned)ctx->numSMs * 8, 256, ctx->streamMain, sc.items, sc.rec, sc.recItem, sc.words, sc.ctl, rg, box);
     if (rc) return rc;
     rc = launch(ctx, ctx->fn[K_QUERY_SCAN], 1, 1024, ctx->streamMain, sc.words, sc.ctl); if (rc) return rc;
-    CU(D(cuEventRecord)(ctx->evEnd, ctx->streamMain));
-    CU(D(cuMemcpyDtoHAsync)(ctx->hExportCtl, sc.ctl, sizeof(QueryCtl), ctx->streamMain));
-    CU(D(cuStreamSynchronize)(ctx->streamMain));
-    const QueryCtl c = *(const QueryCtl*)ctx->hExportCtl;
+    QueryCtl c;
     float ms = 0.0f;
-    CU(D(cuEventElapsedTime)(&ms, ctx->evStart, ctx->evEnd));
+    rc = clock.finish(&ms, {{sc.ctl, &c, sizeof c}}); if (rc) return rc;
     if (kernel_ms) *kernel_ms = ms;
     if (c.plan.error) return failInconsistent(c.plan.error);
     info->num_samples = c.outSamples; info->num_points = c.outPoints; info->num_voxels = c.outVoxels;
@@ -1656,13 +1693,11 @@ int simlod_query_region(SimlodContext* ctx, const SimlodRegion* region, int32_t 
     if (!c.outSamples) return SIMLOD_OK;
     // stage 2: the passing samples into the destination
     CUdeviceptr ds = (CUdeviceptr)dst_samples;
-    CU(D(cuEventRecord)(ctx->evTotalStart, ctx->streamMain));
+    StageClock write(ctx); rc = write.mark(); if (rc) return rc;
     rc = launch(ctx, ctx->fn[K_QUERY_WRITE], (unsigned)ctx->numSMs * 8, 256, ctx->streamMain, sc.items, sc.words, ds, sc.ctl, rg, box);
     if (rc) return rc;
-    CU(D(cuEventRecord)(ctx->evTotalEnd, ctx->streamMain));
-    CU(D(cuEventSynchronize)(ctx->evTotalEnd));
     float writeMs = 0.0f;
-    CU(D(cuEventElapsedTime)(&writeMs, ctx->evTotalStart, ctx->evTotalEnd));
+    rc = write.finish(&writeMs); if (rc) return rc;
     if (kernel_ms) *kernel_ms = ms + writeMs;
     return SIMLOD_OK;
 }
@@ -1688,66 +1723,58 @@ int simlod_pick(SimlodContext* ctx, const uint32_t* pixels, uint64_t num_pixels,
     } else if (num_pixels) {
         return fail(SIMLOD_ERR_INVALID, "num_pixels without a pixel list");
     }
-    if (dst_index % 8 || dst_samples % 16) return fail(SIMLOD_ERR_INVALID, "pick destinations must be 8-byte (indices) and 16-byte (samples) aligned");
+    rc = checkAligned("pick", {{"dst_index", dst_index, 8}, {"dst_samples", dst_samples, 16}}); if (rc) return rc;
     const uint32_t n = (uint32_t)(pixels ? num_pixels : frame);
     // stage 1: the view export's plan, into its scratch, and the one host round trip for its control word
     ExportPlanned p;
-    rc = exportPlan(ctx, -1, &ctx->uniforms, &p);
-    if (kernel_ms) *kernel_ms = p.ms;
-    if (rc) return rc;
+    rc = exportPlan(ctx, -1, &ctx->uniforms, &p, kernel_ms); if (rc) return rc;
     // stage 2: the two frames, then the indices of the requested pixels
-    rc = growDevice(&ctx->pickScratch, &ctx->pickScratchBytes, 16 * frame + 16 + 4ull * n); if (rc) return rc;
-    const CUdeviceptr base = ctx->pickScratch, list = pixels ? base + 16 * frame + 16 : 0;
+    Layout l;
+    const uint64_t oKey = l.take(8 * frame), oIndex = l.take(8 * frame), oHits = l.take(8), oList = l.take(4ull * n);
+    rc = growDevice(&ctx->queryScratch, &ctx->queryScratchBytes, l.bytes); if (rc) return rc;
+    const CUdeviceptr base = ctx->queryScratch, list = pixels ? base + oList : 0;
     if (pixels) CU(D(cuMemcpyHtoDAsync)(list, ids.data(), 4ull * n, ctx->streamMain));
-    PickArgs a{devPtr(p.s.rec), devPtr(p.s.recItem), devPtr(p.s.items), devPtr(base), devPtr(base + 8 * frame), devPtr(base + 16 * frame),
+    PickArgs a{devPtr(p.s.rec), devPtr(p.s.recItem), devPtr(p.s.items), devPtr(base + oKey), devPtr(base + oIndex), devPtr(base + oHits),
                p.c.numItems, p.c.numNodes, 0};
     SimlodUniforms u = ctx->uniforms;
     CUdeviceptr di = (CUdeviceptr)dst_index, ds = (CUdeviceptr)dst_samples;
     uint32_t count = n;
     const unsigned blocks = (unsigned)ctx->numSMs * 4;
-    CU(D(cuEventRecord)(ctx->evStart, ctx->streamMain));
+    StageClock clock(ctx); rc = clock.mark(); if (rc) return rc;
     rc = launch(ctx, ctx->fn[K_PICK_CLEAR], blocks, 256, ctx->streamMain, u, a); if (rc) return rc;
     rc = launch(ctx, ctx->fn[K_PICK_KEY], blocks, 256, ctx->streamMain, u, a); if (rc) return rc;
-    CU(D(cuEventRecord)(ctx->evEnd, ctx->streamMain));
+    rc = clock.mark(); if (rc) return rc;
     rc = launch(ctx, ctx->fn[K_PICK_INDEX], blocks, 256, ctx->streamMain, u, a); if (rc) return rc;
-    CU(D(cuEventRecord)(ctx->evTotalStart, ctx->streamMain));
+    rc = clock.mark(); if (rc) return rc;
     rc = launch(ctx, ctx->fn[K_PICK_WRITE], blocks, 256, ctx->streamMain, a, list, count, di, ds); if (rc) return rc;
-    CU(D(cuEventRecord)(ctx->evTotalEnd, ctx->streamMain));
     uint64_t hits = 0;
-    CU(D(cuMemcpyDtoHAsync)(ctx->hExportCtl, base + 16 * frame, 8, ctx->streamMain));
-    CU(D(cuStreamSynchronize)(ctx->streamMain));
-    memcpy(&hits, ctx->hExportCtl, 8);
-    float keyMs = 0.0f, indexMs = 0.0f, writeMs = 0.0f;
-    CU(D(cuEventElapsedTime)(&keyMs, ctx->evStart, ctx->evEnd));
-    CU(D(cuEventElapsedTime)(&indexMs, ctx->evEnd, ctx->evTotalStart));
-    CU(D(cuEventElapsedTime)(&writeMs, ctx->evTotalStart, ctx->evTotalEnd));
+    float ms[3] = {};                                           // key, index, write
+    rc = clock.finish(ms, {{base + oHits, &hits, sizeof hits}}); if (rc) return rc;
     info->num_hits = hits; info->num_samples = p.c.numSamples; info->num_nodes = p.c.numNodes; info->num_pixels = n;
-    info->plan_ms = p.ms; info->key_ms = keyMs; info->index_ms = indexMs; info->write_ms = writeMs;
-    if (kernel_ms) *kernel_ms = p.ms + keyMs + indexMs + writeMs;
+    info->plan_ms = p.ms; info->key_ms = ms[0]; info->index_ms = ms[1]; info->write_ms = ms[2];
+    if (kernel_ms) *kernel_ms = p.ms + ms[0] + ms[1] + ms[2];
     return SIMLOD_OK;
 }
 
 // ---- k nearest samples (DESIGN.md §9.10); kernels in nearest.cu, the plan is the export's -------------------------------
 namespace {
-// The queries bucketed by home record (nearest.cu's locate, scan and scatter), in the context's nearest scratch: per query
+// The queries bucketed by home record (nearest.cu's locate, scan and scatter), in the context's query scratch: per query
 // home | slot | bucket, per home count | offset | run start, NearestCtl, then `extraBytes` for the caller at *extra.
 // Fills the NearestArgs of the bucketing (no destinations) and enqueues its clears and three kernels.
 int launchBuckets(SimlodContext* ctx, const ExportPlanned& p, uint64_t queries, uint32_t n, int32_t depth, uint64_t extraBytes,
                   NearestArgs* out, CUdeviceptr* extra) {
-    const uint32_t records = p.c.numNodes, homes = records + 1;
-    uint64_t at = 0;
-    auto take = [&](uint64_t bytes) { const uint64_t off = at; at += align16(bytes); return off; };
-    const uint64_t oHome = take(4ull * n), oSlot = take(4ull * n), oBucket = take(4ull * n);
-    const uint64_t oCount = take(4ull * homes), oOffset = take(4ull * homes), oRun = take(4ull * (homes + 1)), oCtl = take(sizeof(NearestCtl));
-    const uint64_t oExtra = take(extraBytes);
-    int rc = growDevice(&ctx->nearestScratch, &ctx->nearestScratchBytes, at); if (rc) return rc;
-    const CUdeviceptr base = ctx->nearestScratch;
-    NearestArgs a{};
-    a.rec = devPtr(p.s.rec); a.recItem = devPtr(p.s.recItem); a.items = devPtr(p.s.items); a.queries = devPtr(queries);
+    const uint32_t homes = p.c.numNodes + 1;
+    Layout l;
+    const uint64_t oHome = l.take(4ull * n), oSlot = l.take(4ull * n), oBucket = l.take(4ull * n);
+    const uint64_t oCount = l.take(4ull * homes), oOffset = l.take(4ull * homes), oRun = l.take(4ull * (homes + 1)), oCtl = l.take(sizeof(NearestCtl));
+    const uint64_t oExtra = l.take(extraBytes);
+    int rc = growDevice(&ctx->queryScratch, &ctx->queryScratchBytes, l.bytes); if (rc) return rc;
+    const CUdeviceptr base = ctx->queryScratch;
+    NearestArgs a = planArgs<NearestArgs>(p, ctx->uniforms, depth);
+    a.queries = devPtr(queries);
     a.home = devPtr(base + oHome); a.slot = devPtr(base + oSlot); a.bucket = devPtr(base + oBucket);
     a.count = devPtr(base + oCount); a.offset = devPtr(base + oOffset); a.runStart = devPtr(base + oRun); a.ctl = devPtr(base + oCtl);
-    a.numQueries = n; a.numRecords = records; a.k = 1; a.depth = depth < 0 ? -1 : depth; a.maxRadius = INFINITY;
-    for (int ax = 0; ax < 3; ax++) { a.boxMin[ax] = ctx->uniforms.boxMin[ax]; a.boxMax[ax] = ctx->uniforms.boxMax[ax]; }
+    a.numQueries = n; a.k = 1; a.maxRadius = INFINITY;
     *out = a;
     if (extra) *extra = base + oExtra;
     const unsigned blocks = (unsigned)std::min<uint64_t>((n + 255) / 256, (uint64_t)ctx->numSMs * 8);
@@ -1772,40 +1799,31 @@ int simlod_query_nearest(SimlodContext* ctx, uint64_t queries, uint64_t num_quer
     if (k < 1 || k > SIMLOD_NEAREST_MAX_K) return fail(SIMLOD_ERR_INVALID, "k = %u, 1 to %d are supported", k, (int)SIMLOD_NEAREST_MAX_K);
     if (num_queries == 0 || num_queries > SIMLOD_NEAREST_MAX_QUERIES)
         return fail(SIMLOD_ERR_INVALID, "%llu queries, 1 to %u are supported", (unsigned long long)num_queries, (unsigned)SIMLOD_NEAREST_MAX_QUERIES);
-    if (depth > SIMLOD_MAX_DEPTH) return fail(SIMLOD_ERR_INVALID, "nearest depth %d exceeds the octree's maximum depth %d", depth, (int)SIMLOD_MAX_DEPTH);
+    rc = checkDepth("nearest", depth); if (rc) return rc;
     if (std::isnan(max_radius) || max_radius < 0.0f) return fail(SIMLOD_ERR_INVALID, "max_radius must be >= 0 or +inf");
-    if (!queries || queries % 16) return fail(SIMLOD_ERR_INVALID, "the query array must be a 16-byte aligned device address");
-    if (dst_index % 8 || dst_dist2 % 4 || dst_samples % 16)
-        return fail(SIMLOD_ERR_INVALID, "nearest destinations must be 8-byte (indices), 4-byte (distances) and 16-byte (samples) aligned");
+    rc = checkAligned("nearest", {{"queries", queries, 16, true}, {"dst_index", dst_index, 8}, {"dst_dist2", dst_dist2, 4}, {"dst_samples", dst_samples, 16}}); if (rc) return rc;
     const uint32_t n = (uint32_t)num_queries;
     // stage 1: the export's plan and chunk items, into its scratch, and the one host round trip for its control word
     ExportPlanned p;
-    rc = exportPlan(ctx, depth < 0 ? -1 : depth, nullptr, &p);
-    if (kernel_ms) *kernel_ms = p.ms;
-    if (rc) return rc;
+    rc = exportPlan(ctx, depth < 0 ? -1 : depth, nullptr, &p, kernel_ms); if (rc) return rc;
     // stage 2: locate and bucket the queries; stage 3: the search, which writes the destinations unless the scan found
     // the record tree inconsistent
-    CU(D(cuEventRecord)(ctx->evStart, ctx->streamMain));
+    StageClock clock(ctx); rc = clock.mark(); if (rc) return rc;
     NearestArgs a{};
     rc = launchBuckets(ctx, p, queries, n, depth, 0, &a, nullptr); if (rc) return rc;
     a.dstIndex = devPtr(dst_index); a.dstDist2 = devPtr(dst_dist2); a.dstSamples = devPtr(dst_samples);
     a.k = k; a.maxRadius = max_radius;
-    CU(D(cuEventRecord)(ctx->evEnd, ctx->streamMain));
+    rc = clock.mark(); if (rc) return rc;
     rc = launch(ctx, ctx->fn[K_NEAREST_SEARCH], searchRuns(n, p.c.numNodes), NEAREST_RUN * 32, ctx->streamMain, a); if (rc) return rc;
-    CU(D(cuEventRecord)(ctx->evTotalEnd, ctx->streamMain));
-    CU(D(cuMemcpyDtoHAsync)(ctx->hExportCtl, (CUdeviceptr)(uintptr_t)a.ctl, sizeof(NearestCtl), ctx->streamMain));
-    CU(D(cuStreamSynchronize)(ctx->streamMain));
     NearestCtl c;
-    memcpy(&c, ctx->hExportCtl, sizeof(c));
-    float bucketMs = 0.0f, searchMs = 0.0f;
-    CU(D(cuEventElapsedTime)(&bucketMs, ctx->evStart, ctx->evEnd));
-    CU(D(cuEventElapsedTime)(&searchMs, ctx->evEnd, ctx->evTotalEnd));
-    if (kernel_ms) *kernel_ms = p.ms + bucketMs + searchMs;
+    float ms[2] = {};                                           // bucket, search
+    rc = clock.finish(ms, {{(CUdeviceptr)(uintptr_t)a.ctl, &c, sizeof c}}); if (rc) return rc;
+    if (kernel_ms) *kernel_ms = p.ms + ms[0] + ms[1];
     if (c.error) return failInconsistent(c.error);
     *info = SimlodNearestInfo{};
     info->num_samples = p.c.numSamples; info->num_found = c.numFound; info->samples_tested = c.samplesTested;
     info->records_visited = c.recordsVisited; info->num_queries = n; info->k = k; info->invalid_queries = (uint32_t)c.invalid;
-    info->max_level = p.c.maxLevel; info->plan_ms = p.ms; info->bucket_ms = bucketMs; info->search_ms = searchMs;
+    info->max_level = p.c.maxLevel; info->plan_ms = p.ms; info->bucket_ms = ms[0]; info->search_ms = ms[1];
     return SIMLOD_OK;
 }
 
@@ -1818,60 +1836,47 @@ int simlod_query_radius(SimlodContext* ctx, uint64_t queries, uint64_t num_queri
     if (!std::isfinite(radius) || radius < 0.0f) return fail(SIMLOD_ERR_INVALID, "radius must be finite and >= 0");
     if (num_queries == 0 || num_queries > SIMLOD_RADIUS_MAX_QUERIES)
         return fail(SIMLOD_ERR_INVALID, "%llu queries, 1 to %u are supported", (unsigned long long)num_queries, (unsigned)SIMLOD_RADIUS_MAX_QUERIES);
-    if (depth > SIMLOD_MAX_DEPTH) return fail(SIMLOD_ERR_INVALID, "radius depth %d exceeds the octree's maximum depth %d", depth, (int)SIMLOD_MAX_DEPTH);
-    if (!queries || queries % 16) return fail(SIMLOD_ERR_INVALID, "the query array must be a 16-byte aligned device address");
-    if (dst_offsets % 8 || dst_index % 8 || dst_dist2 % 4 || dst_samples % 16)
-        return fail(SIMLOD_ERR_INVALID, "radius destinations must be 8-byte (offsets, indices), 4-byte (distances) and 16-byte (samples) aligned");
+    rc = checkDepth("radius", depth); if (rc) return rc;
+    rc = checkAligned("radius", {{"queries", queries, 16, true}, {"dst_offsets", dst_offsets, 8}, {"dst_index", dst_index, 8},
+                                 {"dst_dist2", dst_dist2, 4}, {"dst_samples", dst_samples, 16}}); if (rc) return rc;
     const uint32_t n = (uint32_t)num_queries;
     const bool sizeQuery = !dst_index && !dst_dist2 && !dst_samples;
     // stage 1: the export's plan and chunk items, into its scratch, and the one host round trip for its control word
     ExportPlanned p;
-    rc = exportPlan(ctx, depth < 0 ? -1 : depth, nullptr, &p);
-    if (kernel_ms) *kernel_ms = p.ms;
-    if (rc) return rc;
+    rc = exportPlan(ctx, depth < 0 ? -1 : depth, nullptr, &p, kernel_ms); if (rc) return rc;
     // stage 2: locate and bucket the queries (nearest.cu); stage 3: count, reduce and scan, then one host round trip
     const uint32_t tiles = (n + RADIUS_SCAN_TILE - 1) / RADIUS_SCAN_TILE;
-    uint64_t at = 0;
-    auto take = [&](uint64_t bytes) { const uint64_t off = at; at += align16(bytes); return off; };
-    const uint64_t oCtl = take(sizeof(RadiusCtl)), oTotal = take(4ull * n), oBefore = take(4ull * n), oTile = take(8ull * tiles);
-    const uint64_t oOffsets = take(8ull * (n + 1));
-    CU(D(cuEventRecord)(ctx->evStart, ctx->streamMain));
+    Layout l;
+    const uint64_t oCtl = l.take(sizeof(RadiusCtl)), oTotal = l.take(4ull * n), oBefore = l.take(4ull * n), oTile = l.take(8ull * tiles),
+                   oOffsets = l.take(8ull * (n + 1));
+    StageClock clock(ctx); rc = clock.mark(); if (rc) return rc;
     NearestArgs na{};
     CUdeviceptr base = 0;
-    rc = launchBuckets(ctx, p, queries, n, depth, at, &na, &base); if (rc) return rc;
-    RadiusArgs a{};
-    a.rec = na.rec; a.recItem = na.recItem; a.items = na.items; a.queries = na.queries;
+    rc = launchBuckets(ctx, p, queries, n, depth, l.bytes, &na, &base); if (rc) return rc;
+    RadiusArgs a = planArgs<RadiusArgs>(p, ctx->uniforms, depth);
+    a.queries = devPtr(queries);
     a.count = na.count; a.offset = na.offset; a.runStart = na.runStart; a.bucket = na.bucket; a.nearestCtl = na.ctl;
     a.ctl = devPtr(base + oCtl); a.total = devPtr(base + oTotal); a.before = devPtr(base + oBefore); a.tileSum = devPtr(base + oTile);
     a.offsets = devPtr(base + oOffsets);
     a.dstIndex = devPtr(dst_index); a.dstDist2 = devPtr(dst_dist2); a.dstSamples = devPtr(dst_samples);
-    a.numQueries = n; a.numRecords = p.c.numNodes; a.depth = na.depth; a.radius = radius;
-    for (int ax = 0; ax < 3; ax++) { a.boxMin[ax] = na.boxMin[ax]; a.boxMax[ax] = na.boxMax[ax]; }
+    a.numQueries = n; a.radius = radius;
     CU(D(cuMemsetD8Async)(base + oCtl, 0, sizeof(RadiusCtl), ctx->streamMain));
-    CU(D(cuEventRecord)(ctx->evEnd, ctx->streamMain));
+    rc = clock.mark(); if (rc) return rc;
     const unsigned runs = searchRuns(n, p.c.numNodes);
     rc = launch(ctx, ctx->fn[K_RADIUS_COUNT], runs, NEAREST_RUN * 32, ctx->streamMain, a); if (rc) return rc;
     rc = launch(ctx, ctx->fn[K_RADIUS_REDUCE], tiles, 1024, ctx->streamMain, a); if (rc) return rc;
     rc = launch(ctx, ctx->fn[K_RADIUS_SCAN], tiles, 1024, ctx->streamMain, a); if (rc) return rc;
-    CU(D(cuEventRecord)(ctx->evTotalEnd, ctx->streamMain));
-    uint8_t* const hc = (uint8_t*)ctx->hExportCtl;
-    CU(D(cuMemcpyDtoHAsync)(hc, (CUdeviceptr)(uintptr_t)na.ctl, sizeof(NearestCtl), ctx->streamMain));
-    CU(D(cuMemcpyDtoHAsync)(hc + sizeof(NearestCtl), base + oCtl, sizeof(RadiusCtl), ctx->streamMain));
-    CU(D(cuStreamSynchronize)(ctx->streamMain));
     NearestCtl nc;
     RadiusCtl c;
-    memcpy(&nc, hc, sizeof(nc));
-    memcpy(&c, hc + sizeof(NearestCtl), sizeof(c));
-    float bucketMs = 0.0f, countMs = 0.0f;
-    CU(D(cuEventElapsedTime)(&bucketMs, ctx->evStart, ctx->evEnd));
-    CU(D(cuEventElapsedTime)(&countMs, ctx->evEnd, ctx->evTotalEnd));
-    if (kernel_ms) *kernel_ms = p.ms + bucketMs + countMs;
+    float ms[2] = {};                                           // bucket, count
+    rc = clock.finish(ms, {{(CUdeviceptr)(uintptr_t)na.ctl, &nc, sizeof nc}, {base + oCtl, &c, sizeof c}}); if (rc) return rc;
+    if (kernel_ms) *kernel_ms = p.ms + ms[0] + ms[1];
     if (nc.error) return failInconsistent(nc.error);
     *info = SimlodRadiusInfo{};
     info->num_samples = p.c.numSamples; info->num_found = c.numFound; info->samples_tested = c.samplesTested;
     info->records_visited = c.recordsVisited; info->num_queries = n; info->invalid_queries = (uint32_t)c.invalid;
     info->max_level = p.c.maxLevel; info->max_found = c.maxFound;
-    info->plan_ms = p.ms; info->bucket_ms = bucketMs; info->count_ms = countMs;
+    info->plan_ms = p.ms; info->bucket_ms = ms[0]; info->count_ms = ms[1];
     if (sizeQuery) {                                            // size query: the offsets at most
         if (dst_offsets) {
             CU(D(cuMemcpyDtoDAsync)((CUdeviceptr)dst_offsets, base + oOffsets, 8ull * (n + 1), ctx->streamMain));
@@ -1882,15 +1887,13 @@ int simlod_query_radius(SimlodContext* ctx, uint64_t queries, uint64_t num_queri
     if (capacity < c.numFound)
         return fail(SIMLOD_ERR_INVALID, "radius destinations hold %llu neighbours, the query finds %llu", (unsigned long long)capacity, (unsigned long long)c.numFound);
     // stage 4: the offsets, and the write pass, which places every neighbour
-    CU(D(cuEventRecord)(ctx->evTotalStart, ctx->streamMain));
+    StageClock write(ctx); rc = write.mark(); if (rc) return rc;
     if (dst_offsets) CU(D(cuMemcpyDtoDAsync)((CUdeviceptr)dst_offsets, base + oOffsets, 8ull * (n + 1), ctx->streamMain));
     rc = launch(ctx, ctx->fn[K_RADIUS_WRITE], runs, NEAREST_RUN * 32, ctx->streamMain, a); if (rc) return rc;
-    CU(D(cuEventRecord)(ctx->evTotalEnd, ctx->streamMain));
-    CU(D(cuEventSynchronize)(ctx->evTotalEnd));
     float writeMs = 0.0f;
-    CU(D(cuEventElapsedTime)(&writeMs, ctx->evTotalStart, ctx->evTotalEnd));
+    rc = write.finish(&writeMs); if (rc) return rc;
     info->write_ms = writeMs;
-    if (kernel_ms) *kernel_ms = p.ms + bucketMs + countMs + writeMs;
+    if (kernel_ms) *kernel_ms = p.ms + ms[0] + ms[1] + writeMs;
     return SIMLOD_OK;
 }
 
@@ -1902,36 +1905,27 @@ int simlod_query_ray(SimlodContext* ctx, uint64_t rays, uint64_t num_rays, float
     if (!std::isfinite(radius) || radius < 0.0f) return fail(SIMLOD_ERR_INVALID, "radius must be finite and >= 0");
     if (num_rays == 0 || num_rays > SIMLOD_RAY_MAX_RAYS)
         return fail(SIMLOD_ERR_INVALID, "%llu rays, 1 to %u are supported", (unsigned long long)num_rays, (unsigned)SIMLOD_RAY_MAX_RAYS);
-    if (depth > SIMLOD_MAX_DEPTH) return fail(SIMLOD_ERR_INVALID, "ray depth %d exceeds the octree's maximum depth %d", depth, (int)SIMLOD_MAX_DEPTH);
-    if (!rays || rays % 16) return fail(SIMLOD_ERR_INVALID, "the ray array must be a 16-byte aligned device address");
-    if (dst_index % 8 || dst_t % 4 || dst_h2 % 4 || dst_samples % 16)
-        return fail(SIMLOD_ERR_INVALID, "ray destinations must be 8-byte (indices), 4-byte (t, h2) and 16-byte (samples) aligned");
+    rc = checkDepth("ray", depth); if (rc) return rc;
+    rc = checkAligned("ray", {{"rays", rays, 16, true}, {"dst_index", dst_index, 8}, {"dst_t", dst_t, 4}, {"dst_h2", dst_h2, 4},
+                              {"dst_samples", dst_samples, 16}}); if (rc) return rc;
     const uint32_t n = (uint32_t)num_rays;
     // stage 1: the export's plan and chunk items, into its scratch, and the one host round trip for its control word
     ExportPlanned p;
-    rc = exportPlan(ctx, depth < 0 ? -1 : depth, nullptr, &p);
-    if (kernel_ms) *kernel_ms = p.ms;
-    if (rc) return rc;
-    rc = growDevice(&ctx->rayCtl, &ctx->rayCtlBytes, sizeof(RayCtl)); if (rc) return rc;
-    RayArgs a{};
-    a.rec = devPtr(p.s.rec); a.recItem = devPtr(p.s.recItem); a.items = devPtr(p.s.items); a.rays = devPtr(rays);
-    a.ctl = devPtr(ctx->rayCtl);
+    rc = exportPlan(ctx, depth < 0 ? -1 : depth, nullptr, &p, kernel_ms); if (rc) return rc;
+    rc = growDevice(&ctx->queryScratch, &ctx->queryScratchBytes, sizeof(RayCtl)); if (rc) return rc;
+    RayArgs a = planArgs<RayArgs>(p, ctx->uniforms, depth);
+    a.rays = devPtr(rays); a.ctl = devPtr(ctx->queryScratch);
     a.dstIndex = devPtr(dst_index); a.dstT = devPtr(dst_t); a.dstH2 = devPtr(dst_h2); a.dstSamples = devPtr(dst_samples);
-    a.numRays = n; a.numRecords = p.c.numNodes; a.depth = depth < 0 ? -1 : depth; a.radius = radius;
-    for (int ax = 0; ax < 3; ax++) { a.boxMin[ax] = ctx->uniforms.boxMin[ax]; a.boxMax[ax] = ctx->uniforms.boxMax[ax]; }
+    a.numRays = n; a.radius = radius;
     // stage 2: the level check, then the trace, which writes the destinations unless the check found the record tree
     // inconsistent
-    CU(D(cuEventRecord)(ctx->evStart, ctx->streamMain));
-    CU(D(cuMemsetD8Async)(ctx->rayCtl, 0, sizeof(RayCtl), ctx->streamMain));
+    StageClock clock(ctx); rc = clock.mark(); if (rc) return rc;
+    CU(D(cuMemsetD8Async)(ctx->queryScratch, 0, sizeof(RayCtl), ctx->streamMain));
     rc = launch(ctx, ctx->fn[K_RAY_CHECK], 1, 1024, ctx->streamMain, a); if (rc) return rc;
     rc = launch(ctx, ctx->fn[K_RAY_TRACE], (n + RAY_WARPS - 1) / RAY_WARPS, RAY_WARPS * 32, ctx->streamMain, a); if (rc) return rc;
-    CU(D(cuEventRecord)(ctx->evEnd, ctx->streamMain));
-    CU(D(cuMemcpyDtoHAsync)(ctx->hExportCtl, ctx->rayCtl, sizeof(RayCtl), ctx->streamMain));
-    CU(D(cuStreamSynchronize)(ctx->streamMain));
     RayCtl c;
-    memcpy(&c, ctx->hExportCtl, sizeof(c));
     float traceMs = 0.0f;
-    CU(D(cuEventElapsedTime)(&traceMs, ctx->evStart, ctx->evEnd));
+    rc = clock.finish(&traceMs, {{ctx->queryScratch, &c, sizeof c}}); if (rc) return rc;
     if (kernel_ms) *kernel_ms = p.ms + traceMs;
     if (c.error) return failInconsistent(c.error);
     *info = SimlodRayInfo{};
@@ -2378,9 +2372,9 @@ int writeLas(SimlodContext* ctx, const char* path, const SimlodLasWriteParams* p
         if (!std::isfinite(params->scale[a]) || !(params->scale[a] > 0.0)) return fail(SIMLOD_ERR_INVALID, "LAS scale[%d] = %g must be finite and > 0", a, params->scale[a]);
         if (!std::isfinite(params->offset[a]) || !std::isfinite(params->translation[a])) return fail(SIMLOD_ERR_INVALID, "LAS offset and translation must be finite (axis %d)", a);
     }
-    if (samples % 16) return fail(SIMLOD_ERR_INVALID, "samples must be 16-byte aligned");
+    rc = checkAligned("LAS", {{"samples", samples, 16}}); if (rc) return rc;
     if (samples && depth >= 0) return fail(SIMLOD_ERR_INVALID, "a depth selects a cut of the octree's samples; it does not apply to a caller's array");
-    if (depth > SIMLOD_MAX_DEPTH) return fail(SIMLOD_ERR_INVALID, "LAS depth %d exceeds the octree's maximum depth %d", depth, (int)SIMLOD_MAX_DEPTH);
+    rc = checkDepth("LAS", depth); if (rc) return rc;
     if (samples && numSamples > UINT32_MAX) return fail(SIMLOD_ERR_INVALID, "%llu samples: a LAS 1.2 file holds at most 2^32 - 1 points", (unsigned long long)numSamples);
     if (params->writer_threads < 1 || params->writer_threads > 64) return fail(SIMLOD_ERR_INVALID, "writer_threads %u is outside 1..64", params->writer_threads);
     // written under a temporary name and renamed once complete: a failed call leaves no file and replaces no existing one
