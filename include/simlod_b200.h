@@ -415,6 +415,60 @@ int simlod_query_radius(SimlodContext* ctx, uint64_t queries, uint64_t num_queri
                         uint64_t dst_offsets, uint64_t dst_index, uint64_t dst_dist2, uint64_t dst_samples,
                         uint64_t capacity, SimlodRadiusInfo* info, float* kernel_ms);
 
+// Height maps (DESIGN.md §9.14): per cell of a grid over the x-y plane, the count, lowest, highest and mean z of the
+// samples of a sample set that fall in it, and the highest of them, as an index into the sample array
+// simlod_export_octree(depth) returns for the same state.
+#define SIMLOD_HEIGHTMAP_MAX_CELLS (1u << 27)
+typedef struct SimlodHeightmap {
+    float    origin[2];                             //   0  (ox, oy): the low corner of cell (0, 0)
+    float    cell;                                  //   8  edge of the square cells
+    uint32_t nx, ny;                                //  12  cells per row (x), rows (y)
+    uint32_t reserved;                              //  20
+} SimlodHeightmap;
+SIMLOD_STATIC_ASSERT(sizeof(SimlodHeightmap) == 24, "Heightmap");
+SIMLOD_STATIC_ASSERT(offsetof(SimlodHeightmap, cell) == 8 && offsetof(SimlodHeightmap, nx) == 12, "Heightmap.cell");
+typedef struct SimlodHeightmapInfo {
+    uint64_t num_samples;                           //   0  samples of the export at `depth`: the index space
+    uint64_t num_binned;                            //   8  samples that fell in a cell (the sum of the counts)
+    uint64_t samples_tested;                        //  16  samples read: those of the chunk items the culling kept
+    uint64_t records_visited;                       //  24  records with samples the culling kept
+    uint64_t nonempty_cells;                        //  32
+    uint32_t max_level;                             //  40  deepest level in the octree
+    float    plan_ms, accumulate_ms, finalize_ms;   //  44  event time of the export's plan, of the reset + accumulate,
+                                                    //      and of the finalize (which writes the destinations)
+} SimlodHeightmapInfo;
+SIMLOD_STATIC_ASSERT(sizeof(SimlodHeightmapInfo) == 56, "HeightmapInfo");
+SIMLOD_STATIC_ASSERT(offsetof(SimlodHeightmapInfo, max_level) == 40 && offsetof(SimlodHeightmapInfo, plan_ms) == 44, "HeightmapInfo.max_level");
+//   grid         cell (i, j) is the square [ox + i cell, ox + (i+1) cell) x [oy + j cell, oy + (j+1) cell) as computed
+//                below; results are (ny, nx) arrays, row j, column i, rows in +y order (no image flip)
+//   cell of p    in float32, round to nearest, nothing contracted: u = (x - ox) / cell, v = (y - oy) / cell, both IEEE
+//                divisions. p counts in cell (trunc(u), trunc(v)) when u >= 0 and v >= 0 (a NaN fails; -0 passes) and
+//                trunc(u) < nx, trunc(v) < ny (saturating float -> uint32)
+//   sample set   as simlod_query_nearest's: depth < 0, the eligible points of every leaf (the inserted point set);
+//                0 <= depth <= 20, the export's cut at `depth`, its points eligible ones, its voxels always
+//   z order      the sign-aware bit order of float32 (-0 below +0)
+//   result       per cell: dst_count (int64, 0 when empty), dst_z_min, dst_z_max (float32, NaN 0x7fc00000 when empty),
+//                dst_z_mean (float32, below), dst_top (int64: the index of the highest sample, equal z to the smallest
+//                index; -1 when empty) and dst_samples (the top sample's 16-byte SimlodPoint, bit for bit
+//                export_octree(depth).samples[top]; zeros when empty)
+//   z_mean       fixed point, in double with every operation rounded to nearest and nothing contracted: size = the cube
+//                edge (the largest of boxMax - boxMin in float32), K = 2^30 / size, q = rint_even((z - minz) K) per
+//                sample (z, minz = boxMin[2] widened to double), S = the int64 sum of q over the cell, and
+//                z_mean = float32(minz + (S / n) / K): the mean of z quantised to 2^-30 of the cube edge
+// Each destination may be 0 (not written); with all of them 0 the call fills *info only. SIMLOD_ERR_INVALID before any
+// launch, with nothing written, for a null info or grid, a non-finite origin, a cell that is not finite or not > 0, nx
+// or ny 0, nx * ny above SIMLOD_HEIGHTMAP_MAX_CELLS (tile larger rasters), depth > 20 or a misaligned destination (8
+// bytes for the int64 results, 4 for float32, 16 for samples); after the plan, with nothing written, for an export of
+// 2^32 samples or more and for an inconsistent image (the export's conditions). A record whose lattice box cannot hold a
+// sample of a cell of the grid is skipped unread, so the result equals binning every sample of the set, and two calls on
+// the same state are byte-identical. Reads the ABI only, as the export does, and writes nothing into the context's
+// buffers or Stats. Enqueued on the launch stream; returns once complete. *kernel_ms (optional) = event time of all its
+// kernels. Scratch: the export's, and up to 24 bytes per cell (4 for the count, 4 for z_min, 8 for z_max / top / samples,
+// 8 for z_mean), kept until simlod_destroy.
+int simlod_query_heightmap(SimlodContext* ctx, const SimlodHeightmap* grid, int32_t depth, uint64_t dst_count, uint64_t dst_z_min,
+                           uint64_t dst_z_max, uint64_t dst_z_mean, uint64_t dst_top, uint64_t dst_samples,
+                           SimlodHeightmapInfo* info, float* kernel_ms);
+
 // Octree files (SimlodOctreeFileHeader, DESIGN.md §9.7): a built octree saved and loaded back, so that it can be rendered,
 // exported or continued with new batches in another context, process or session.
 // simlod_read_octree_header: the header of an octree file, checked against itself and the file size. No context, no GPU.

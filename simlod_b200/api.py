@@ -195,6 +195,22 @@ class SimlodRadiusInfo(C.Structure):
                 ("count_ms", C.c_float), ("write_ms", C.c_float)]
 
 
+HEIGHTMAP_MAX_CELLS = 1 << 27
+
+
+class SimlodHeightmap(C.Structure):
+    """SimlodHeightmap: a grid of nx x ny square cells of edge `cell` over the x-y plane, cell (0, 0) at `origin`."""
+    _fields_ = [("origin", C.c_float * 2), ("cell", C.c_float), ("nx", C.c_uint32), ("ny", C.c_uint32), ("reserved", C.c_uint32)]
+
+
+class SimlodHeightmapInfo(C.Structure):
+    """SimlodHeightmapInfo: the export's sample count (the index space), the samples binned (the sum of the counts), how
+    much of the octree the culling left to read, the non-empty cells, and the event time of each stage."""
+    _fields_ = [("num_samples", C.c_uint64), ("num_binned", C.c_uint64), ("samples_tested", C.c_uint64),
+                ("records_visited", C.c_uint64), ("nonempty_cells", C.c_uint64), ("max_level", C.c_uint32),
+                ("plan_ms", C.c_float), ("accumulate_ms", C.c_float), ("finalize_ms", C.c_float)]
+
+
 class LasWriteParams(C.Structure):
     """SimlodLasWriteParams: the file's scale and offset, the translation added to every sample, the writer threads."""
     _fields_ = [("scale", C.c_double * 3), ("offset", C.c_double * 3), ("translation", C.c_double * 3),
@@ -258,6 +274,7 @@ assert C.sizeof(OctreeFileHeader) == 128
 assert C.sizeof(SimlodRegion) == 304 and C.sizeof(SimlodQueryInfo) == 40
 assert C.sizeof(SimlodPickInfo) == 40 and C.sizeof(SimlodNearestInfo) == 64 and C.sizeof(SimlodRayInfo) == 56
 assert C.sizeof(SimlodRadiusInfo) == 64
+assert C.sizeof(SimlodHeightmap) == 24 and C.sizeof(SimlodHeightmapInfo) == 56
 assert C.sizeof(LasWriteParams) == 80 and C.sizeof(LasWriteInfo) == 96
 
 # every symbol include/simlod_b200.h declares
@@ -273,6 +290,7 @@ EXPORTS = [
     "simlod_export_octree", "simlod_export_view", "simlod_read_las_header", "simlod_insert_files",
     "simlod_read_octree_header", "simlod_save_octree", "simlod_load_octree", "simlod_query_region",
     "simlod_pick", "simlod_query_nearest", "simlod_query_ray", "simlod_query_radius", "simlod_write_las", "simlod_files_box",
+    "simlod_query_heightmap",
 ]
 
 _lib = None
@@ -345,6 +363,8 @@ def load_library():
         "simlod_write_las": [vp, C.c_char_p, C.POINTER(LasWriteParams), u64, u64, C.c_int32, C.POINTER(LasWriteInfo),
                              C.POINTER(C.c_float)],
         "simlod_files_box": [C.POINTER(C.c_char_p), u32, C.POINTER(C.c_float), C.POINTER(C.c_float)],
+        "simlod_query_heightmap": [vp, C.POINTER(SimlodHeightmap), C.c_int32, u64, u64, u64, u64, u64, u64,
+                                   C.POINTER(SimlodHeightmapInfo), C.POINTER(C.c_float)],
     }
     for name, argtypes in sig.items():
         fn = getattr(lib, name)
@@ -1031,6 +1051,36 @@ class SimLOD:
         with _DeviceInput(self, r) as rptr, _Results(self, device, (((n,), I8), ((n,), F4), ((n,), F4), ((n,), POINT_DTYPE) if samples else None)) as out:
             info, _ = self.query_ray_into(rptr, n, radius, depth, *out.ptrs)
             return out.results() + (info,)
+
+    def query_heightmap_into(self, grid, depth, dst_count, dst_z_min, dst_z_max, dst_z_mean, dst_top, dst_samples):
+        """simlod_query_heightmap on caller-owned device memory: `grid` a SimlodHeightmap, destinations [ny][nx] int64 /
+        float32 / float32 / float32 / int64 / 16-byte samples, each 0 for not written (depth None or < 0: the inserted
+        points). Returns (SimlodHeightmapInfo, kernel ms)."""
+        return self._call(self._lib.simlod_query_heightmap, SimlodHeightmapInfo(), C.byref(grid), _depth(depth), int(dst_count),
+                          int(dst_z_min), int(dst_z_max), int(dst_z_mean), int(dst_top), int(dst_samples))
+
+    def query_heightmap(self, origin, cell, shape, depth=None, device="cuda", samples=False):
+        """A height map of the stored samples (simlod_query_heightmap), exact: per cell of the grid of square cells of
+        edge `cell` with cell (0, 0) at `origin` (x, y), the samples whose u = (x - ox) / cell and v = (y - oy) / cell
+        (float32, IEEE division) satisfy u >= 0, v >= 0, trunc(u) < nx and trunc(v) < ny fall in cell (trunc(u), trunc(v)).
+        With depth=None the inserted points (those on the cube's max face excepted, as query_region), with an integer
+        depth the samples of export_octree(depth). `shape` is (ny, nx), at most 2^27 cells (tile larger rasters); row j,
+        column i is cell (i, j), rows in +y order. Returns (count, z_min, z_max, z_mean, top, info) or, with
+        samples=True, (count, z_min, z_max, z_mean, top, samples, info): (ny, nx) int64 counts; float32 lowest, highest
+        and mean z, NaN for an empty cell (z ordered by its sign-aware bits, -0 below +0; the mean is that of z
+        quantised to 2^-30 of the cube edge, byte-deterministic); int64 indices into export_octree(depth).samples of the
+        highest sample, equal z to the smallest index, -1 for an empty cell; (ny, nx, 4) float32 samples in the export's
+        layout, zeros for an empty cell. device="cuda": torch tensors in device memory; device="cpu": numpy arrays (the
+        samples as POINT_DTYPE)."""
+        ny, nx = (int(v) for v in shape)
+        if ny < 0 or nx < 0 or ny > 0xFFFFFFFF or nx > 0xFFFFFFFF:
+            raise ValueError("shape must be (ny, nx) with 0 <= nx, ny < 2^32")
+        grid = SimlodHeightmap(cell=float(cell), nx=nx, ny=ny)
+        grid.origin[:] = [float(v) for v in origin]
+        s = (ny, nx)
+        with _Results(self, device, ((s, I8), (s, F4), (s, F4), (s, F4), (s, I8), (s, POINT_DTYPE) if samples else None)) as r:
+            info, _ = self.query_heightmap_into(grid, depth, *r.ptrs)
+            return r.results() + (info,)
 
     def host_alloc(self, nbytes):
         p = C.c_void_p()

@@ -1,6 +1,6 @@
 """Build recipe for the native parts (no torch involved).
 
-  simlod_b200/csrc/{construct,render,reset,util,las,partition,gen,export,import,query,pick,nearest,ray,radius,las_write}.cu  --nvcc sm_90a-->  build/*.cubin
+  simlod_b200/csrc/{construct,render,reset,util,las,partition,gen,export,import,query,pick,nearest,ray,radius,las_write,heightmap}.cu  --nvcc sm_90a-->  build/*.cubin
   build/*.cubin --bin2c--> build/*_cubin.c  (embedded images)
   simlod_b200/csrc/host.cpp + images --g++--> simlod_b200/libsimlod_b200.so   (the C ABI, include/simlod_b200.h)
   build/*.cubin are also copied to simlod_b200/cubin/ : the drop-in artefacts for the reference's
@@ -22,7 +22,7 @@ BIN2C = os.path.join(CUDA, "bin", "bin2c")
 LIB = os.path.join(ROOT, "simlod_b200", "libsimlod_b200.so")
 CUBIN_DIR = os.path.join(ROOT, "simlod_b200", "cubin")
 PROGRAMS = ["construct", "render", "reset", "util", "las", "partition", "gen", "export", "import", "query", "pick", "nearest", "ray", "radius",
-            "las_write"]
+            "las_write", "heightmap"]
 # gen.cu restates numpy generators in IEEE double arithmetic: no mul+add contraction
 EXTRA_FLAGS = {"gen": ["--fmad=false"]}
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]

@@ -56,6 +56,9 @@ __device__ __forceinline__ float max_ftz(float a, float b) {
 }
 // a / b as the reference computes it: a * MUFU.RCP(b), product flushed
 __device__ __forceinline__ float div_fast(float a, float b) { return mul_ftz(a, rcp(b)); }
+__device__ __forceinline__ float div_rn(float a, float b) {    // IEEE a / b, denormals kept: numpy's float32 a / b
+    float r; asm("div.rn.f32 %0, %1, %2;" : "=f"(r) : "f"(a), "f"(b)); return r;
+}
 
 __device__ __forceinline__ uint32_t f2u(float a) {       // F2I.FTZ.U32.TRUNC (saturating, NaN -> 0)
     uint32_t r; asm("cvt.rzi.ftz.u32.f32 %0, %1;" : "=r"(r) : "f"(a)); return r;

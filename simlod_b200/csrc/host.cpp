@@ -53,6 +53,7 @@ extern const unsigned char simlod_cubin_nearest[];
 extern const unsigned char simlod_cubin_ray[];
 extern const unsigned char simlod_cubin_radius[];
 extern const unsigned char simlod_cubin_las_write[];
+extern const unsigned char simlod_cubin_heightmap[];
 }
 
 namespace {
@@ -118,10 +119,11 @@ struct Program {
 
 // The embedded images of the kernels that are launched outside the three swappable programs, and those kernels: one
 // row each, {enum value, image, kernel name}. createResources loads every image and looks up every kernel.
-enum Image { IMG_UTIL, IMG_LAS, IMG_GEN, IMG_PARTITION, IMG_EXPORT, IMG_QUERY, IMG_IMPORT, IMG_PICK, IMG_NEAREST, IMG_RAY, IMG_RADIUS, IMG_LAS_WRITE, NUM_IMAGES };
+enum Image { IMG_UTIL, IMG_LAS, IMG_GEN, IMG_PARTITION, IMG_EXPORT, IMG_QUERY, IMG_IMPORT, IMG_PICK, IMG_NEAREST, IMG_RAY, IMG_RADIUS, IMG_LAS_WRITE, IMG_HEIGHTMAP, NUM_IMAGES };
 const unsigned char* const IMAGES[NUM_IMAGES] = {simlod_cubin_util, simlod_cubin_las, simlod_cubin_gen, simlod_cubin_partition,
                                                  simlod_cubin_export, simlod_cubin_query, simlod_cubin_import, simlod_cubin_pick,
-                                                 simlod_cubin_nearest, simlod_cubin_ray, simlod_cubin_radius, simlod_cubin_las_write};
+                                                 simlod_cubin_nearest, simlod_cubin_ray, simlod_cubin_radius, simlod_cubin_las_write,
+                                                 simlod_cubin_heightmap};
 #define KERNEL_LIST(X)                                                                                    \
     X(K_RCP, IMG_UTIL, "simlod_util_rcp") X(K_FILL, IMG_UTIL, "simlod_util_fill")                         \
     X(K_LAS, IMG_LAS, "simlod_las_decode")                                                                \
@@ -146,7 +148,9 @@ const unsigned char* const IMAGES[NUM_IMAGES] = {simlod_cubin_util, simlod_cubin
     X(K_RAY_CHECK, IMG_RAY, "simlod_ray_check") X(K_RAY_TRACE, IMG_RAY, "simlod_ray_trace")                 \
     X(K_RADIUS_COUNT, IMG_RADIUS, "simlod_radius_count") X(K_RADIUS_REDUCE, IMG_RADIUS, "simlod_radius_reduce") \
     X(K_RADIUS_SCAN, IMG_RADIUS, "simlod_radius_scan") X(K_RADIUS_WRITE, IMG_RADIUS, "simlod_radius_write") \
-    X(K_LAS_ENCODE, IMG_LAS_WRITE, "simlod_las_encode")
+    X(K_LAS_ENCODE, IMG_LAS_WRITE, "simlod_las_encode")                                                   \
+    X(K_HEIGHTMAP_ACCUMULATE, IMG_HEIGHTMAP, "simlod_heightmap_accumulate")                               \
+    X(K_HEIGHTMAP_FINALIZE, IMG_HEIGHTMAP, "simlod_heightmap_finalize")
 #define X(k, image, name) k,
 enum Kernel { KERNEL_LIST(X) NUM_KERNELS };
 #undef X
@@ -212,7 +216,7 @@ struct SimlodContext {
     uint64_t exportScratchBytes = 0;
     void* hExportCtl = nullptr;        // pinned copy of the control structs read back (StageClock::finish)
     CUdeviceptr queryScratch = 0;      // the plan's consumers, one at a time: pick's frames, the buckets and passes of k
-    uint64_t queryScratchBytes = 0;    // nearest and radius, RayCtl
+    uint64_t queryScratchBytes = 0;    // nearest and radius, RayCtl, the height map's accumulators
     CUdeviceptr fileWindow = 0;        // octree files: FILE_WINDOW_BYTES of samples staged on the device
     CUdeviceptr fileTables = 0;        // octree load: records | plan | error word, sized for nodes[]
     CUdeviceptr lasWindow = 0;         // LAS writer: one window of records, then LasWriteCtl
@@ -1462,7 +1466,8 @@ namespace {
 constexpr uint64_t align16(uint64_t v) { return (v + 15) & ~15ull; }
 constexpr size_t CTL_HOST_BYTES = 128;      // the pinned copy of the control word
 static_assert(sizeof(ExportCtl) <= CTL_HOST_BYTES && sizeof(QueryCtl) <= CTL_HOST_BYTES && sizeof(NearestCtl) <= CTL_HOST_BYTES &&
-              sizeof(RayCtl) <= CTL_HOST_BYTES && sizeof(NearestCtl) + sizeof(RadiusCtl) <= CTL_HOST_BYTES, "pinned control word");
+              sizeof(RayCtl) <= CTL_HOST_BYTES && sizeof(NearestCtl) + sizeof(RadiusCtl) <= CTL_HOST_BYTES &&
+              sizeof(HeightmapCtl) <= CTL_HOST_BYTES, "pinned control word");
 
 // Consecutive 16-byte aligned regions of one allocation: take() returns the offset of the next one
 struct Layout { uint64_t bytes = 0; uint64_t take(uint64_t n) { const uint64_t off = bytes; bytes += align16(n); return off; } };
@@ -1585,7 +1590,7 @@ int exportPlan(SimlodContext* ctx, int32_t depth, const SimlodUniforms* view, Ex
     return SIMLOD_OK;
 }
 
-// The fields NearestArgs, RadiusArgs and RayArgs share: the plan's records and chunk items, the cut and the octree cube
+// The fields NearestArgs, RadiusArgs, RayArgs and HeightmapArgs share: the plan's records and chunk items, the cut and the octree cube
 extern "C++" template <class Args> Args planArgs(const ExportPlanned& p, const SimlodUniforms& u, int32_t depth) {
     Args a{};
     a.rec = devPtr(p.s.rec); a.recItem = devPtr(p.s.recItem); a.items = devPtr(p.s.items);
@@ -1932,6 +1937,64 @@ int simlod_query_ray(SimlodContext* ctx, uint64_t rays, uint64_t num_rays, float
     info->num_samples = p.c.numSamples; info->num_hits = c.numHits; info->samples_tested = c.samplesTested;
     info->records_visited = c.recordsVisited; info->num_rays = n; info->invalid_rays = (uint32_t)c.invalid;
     info->max_level = p.c.maxLevel; info->plan_ms = p.ms; info->trace_ms = traceMs;
+    return SIMLOD_OK;
+}
+
+// ---- height maps (DESIGN.md §9.14); kernels in heightmap.cu, the plan is the export's -----------------------------------
+int simlod_query_heightmap(SimlodContext* ctx, const SimlodHeightmap* grid, int32_t depth, uint64_t dst_count, uint64_t dst_z_min,
+                           uint64_t dst_z_max, uint64_t dst_z_mean, uint64_t dst_top, uint64_t dst_samples,
+                           SimlodHeightmapInfo* info, float* kernel_ms) {
+    int rc = setCurrent(ctx); if (rc) return rc;
+    if (!info) return fail(SIMLOD_ERR_INVALID, "null info");
+    if (!grid) return fail(SIMLOD_ERR_INVALID, "null grid");
+    const SimlodHeightmap g = *grid;
+    if (!std::isfinite(g.origin[0]) || !std::isfinite(g.origin[1])) return fail(SIMLOD_ERR_INVALID, "heightmap origin must be finite");
+    if (!std::isfinite(g.cell) || !(g.cell > 0.0f)) return fail(SIMLOD_ERR_INVALID, "heightmap cell must be finite and > 0");
+    const uint64_t cells = (uint64_t)g.nx * g.ny;
+    if (cells == 0 || cells > SIMLOD_HEIGHTMAP_MAX_CELLS)
+        return fail(SIMLOD_ERR_INVALID, "heightmap of %u x %u cells, 1 to %u cells are supported (tile larger rasters)", g.nx, g.ny,
+                    (unsigned)SIMLOD_HEIGHTMAP_MAX_CELLS);
+    rc = checkDepth("heightmap", depth); if (rc) return rc;
+    rc = checkAligned("heightmap", {{"dst_count", dst_count, 8}, {"dst_z_min", dst_z_min, 4}, {"dst_z_max", dst_z_max, 4},
+                                    {"dst_z_mean", dst_z_mean, 4}, {"dst_top", dst_top, 8}, {"dst_samples", dst_samples, 16}}); if (rc) return rc;
+    // stage 1: the export's plan and chunk items, into its scratch, and the one host round trip for its control word
+    ExportPlanned p;
+    rc = exportPlan(ctx, depth < 0 ? -1 : depth, nullptr, &p, kernel_ms); if (rc) return rc;
+    if (p.c.numSamples >> 32)
+        return fail(SIMLOD_ERR_INVALID, "heightmap: the export holds %llu samples, at most 2^32 - 1 are supported", (unsigned long long)p.c.numSamples);
+    // the accumulators a destination needs; the count is always kept, for the info
+    const bool wantMin = dst_z_min, wantTop = dst_z_max || dst_top || dst_samples, wantSum = dst_z_mean;
+    Layout l;
+    const uint64_t oCtl = l.take(sizeof(HeightmapCtl)), oCount = l.take(4 * cells), oMin = l.take(wantMin ? 4 * cells : 0),
+                   oTop = l.take(wantTop ? 8 * cells : 0), oSum = l.take(wantSum ? 8 * cells : 0);
+    rc = growDevice(&ctx->queryScratch, &ctx->queryScratchBytes, l.bytes); if (rc) return rc;
+    const CUdeviceptr base = ctx->queryScratch;
+    HeightmapArgs a = planArgs<HeightmapArgs>(p, ctx->uniforms, depth);
+    a.ctl = devPtr(base + oCtl); a.count = devPtr(base + oCount);
+    a.zmin = devPtr(wantMin ? base + oMin : 0); a.top = devPtr(wantTop ? base + oTop : 0); a.sum = devPtr(wantSum ? base + oSum : 0);
+    a.dstCount = devPtr(dst_count); a.dstZMin = devPtr(dst_z_min); a.dstZMax = devPtr(dst_z_max); a.dstZMean = devPtr(dst_z_mean);
+    a.dstTop = devPtr(dst_top); a.dstSamples = devPtr(dst_samples);
+    a.numItems = p.c.numItems; a.nx = g.nx; a.ny = g.ny;
+    a.origin[0] = g.origin[0]; a.origin[1] = g.origin[1]; a.cell = g.cell;
+    // stage 2: reset the accumulators (memsets) and bin every sample; stage 3: the destinations
+    StageClock clock(ctx); rc = clock.mark(); if (rc) return rc;
+    CU(D(cuMemsetD8Async)(base + oCtl, 0, sizeof(HeightmapCtl), ctx->streamMain));
+    CU(D(cuMemsetD32Async)(base + oCount, 0, cells, ctx->streamMain));
+    if (wantMin) CU(D(cuMemsetD32Async)(base + oMin, 0xffffffffu, cells, ctx->streamMain));
+    if (wantTop) CU(D(cuMemsetD8Async)(base + oTop, 0, 8 * cells, ctx->streamMain));
+    if (wantSum) CU(D(cuMemsetD8Async)(base + oSum, 0, 8 * cells, ctx->streamMain));
+    rc = launch(ctx, ctx->fn[K_HEIGHTMAP_ACCUMULATE], (unsigned)ctx->numSMs * 8, 256, ctx->streamMain, a); if (rc) return rc;
+    rc = clock.mark(); if (rc) return rc;
+    const unsigned blocks = (unsigned)std::min<uint64_t>((cells + 255) / 256, (uint64_t)ctx->numSMs * 8);
+    rc = launch(ctx, ctx->fn[K_HEIGHTMAP_FINALIZE], blocks, 256, ctx->streamMain, a); if (rc) return rc;
+    HeightmapCtl c;
+    float ms[2] = {};                                           // reset + accumulate, finalize
+    rc = clock.finish(ms, {{base + oCtl, &c, sizeof c}}); if (rc) return rc;
+    if (kernel_ms) *kernel_ms = p.ms + ms[0] + ms[1];
+    *info = SimlodHeightmapInfo{};
+    info->num_samples = p.c.numSamples; info->num_binned = c.numBinned; info->samples_tested = c.samplesTested;
+    info->records_visited = c.recordsVisited; info->nonempty_cells = c.nonemptyCells; info->max_level = p.c.maxLevel;
+    info->plan_ms = p.ms; info->accumulate_ms = ms[0]; info->finalize_ms = ms[1];
     return SIMLOD_OK;
 }
 

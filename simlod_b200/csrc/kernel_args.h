@@ -1,6 +1,6 @@
 // kernel_args.h — the argument and control structs that host.cpp fills and the kernels read, with the codes and limits
 // both sides use. One definition for both compilers: plain C++ (no device code), included by host.cpp and by export.cu,
-// query.cu, pick.cu, nearest.cu, radius.cu and ray.cu (through export_common.cuh), import.cu, partition.cu and las_write.cu. The static_asserts pin
+// query.cu, pick.cu, nearest.cu, radius.cu, ray.cu and heightmap.cu (through export_common.cuh), import.cu, partition.cu and las_write.cu. The static_asserts pin
 // every size, and the offsets that one side reads of a struct the other writes, so a layout change fails to compile instead
 // of shifting bytes.
 #pragma once
@@ -158,6 +158,40 @@ struct RayArgs {                          // the export's plan (export scratch),
     float boxMin[3], boxMax[3];           // of the uniforms: the octree cube
 };
 static_assert(sizeof(RayArgs) == 112 && offsetof(RayArgs, numRays) == 72 && offsetof(RayArgs, boxMin) == 88, "RayArgs");
+
+// ---- height maps (heightmap.cu) --------------------------------------------------------------------------------------
+
+struct HeightmapCtl {                     // zeroed by the host before the accumulate; read back after the finalize
+    uint64_t numBinned, samplesTested, recordsVisited;   // summed by the accumulate, in this order
+    uint64_t nonemptyCells;               // summed by the finalize
+};
+static_assert(sizeof(HeightmapCtl) == 32 && offsetof(HeightmapCtl, nonemptyCells) == 24, "HeightmapCtl");
+
+struct HeightmapArgs {                    // the export's plan (export scratch), the per-cell accumulators and the destinations
+    const SimlodExportNode* rec;          // [record] the plan's breadth-first records
+    const uint64_t* recItem;              // [record] first chunk item of the record's point list (its voxel list follows)
+    const uint64_t* items;                // [item] two words: Item {src, dst | count << 48} (export_common.cuh)
+    HeightmapCtl* ctl;
+    uint32_t* count;                      // [cell] binned samples (memset 0)
+    uint32_t* zmin;                       // [cell] the least ordered z (memset 0xff), or null when not needed
+    unsigned long long* top;              // [cell] ordered(z) << 32 | (0xffffffff - index), the largest (memset 0), or null
+    unsigned long long* sum;              // [cell] the sum of the fixed-point z (memset 0), or null
+    int64_t* dstCount;                    // [cell] or null
+    float* dstZMin;                       // [cell] or null
+    float* dstZMax;                       // [cell] or null
+    float* dstZMean;                      // [cell] or null
+    int64_t* dstTop;                      // [cell] or null
+    SimlodPoint* dstSamples;              // [cell] or null
+    uint64_t numItems;
+    uint32_t numRecords;
+    int32_t depth;                        // < 0: the points of the leaves; else the export's cut at `depth`
+    uint32_t nx, ny;                      // cells per row, rows
+    float origin[2], cell;
+    float boxMin[3], boxMax[3];           // of the uniforms: the octree cube
+    uint32_t pad;
+};
+static_assert(sizeof(HeightmapArgs) == 176 && offsetof(HeightmapArgs, numItems) == 112 && offsetof(HeightmapArgs, origin) == 136 &&
+              offsetof(HeightmapArgs, boxMin) == 148, "HeightmapArgs");
 
 // ---- LAS writer (las_write.cu) ---------------------------------------------------------------------------------------
 
