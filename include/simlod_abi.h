@@ -270,3 +270,26 @@ SIMLOD_STATIC_ASSERT(offsetof(SimlodOctreeFileHeader, counters_offset) == 96, "O
 SIMLOD_STATIC_ASSERT(offsetof(SimlodOctreeFileHeader, samples_offset) == 104, "OctreeFileHeader.samples_offset");
 SIMLOD_STATIC_ASSERT(offsetof(SimlodOctreeFileHeader, file_size) == 112, "OctreeFileHeader.file_size");
 SIMLOD_STATIC_ASSERT(offsetof(SimlodOctreeFileHeader, reserved1) == 120, "OctreeFileHeader.reserved1");
+
+// Region query and clip volumes (simlod_b200.h, DESIGN.md §9.8 and §9.15): kernel arguments of query.cu, render.cu and
+// pick.cu
+enum { SIMLOD_REGION_BOX = 1, SIMLOD_REGION_SPHERE = 2, SIMLOD_REGION_PLANES = 3 };
+#define SIMLOD_REGION_MAX_PLANES 16
+typedef struct SimlodRegion {
+    uint32_t kind, num_planes;                      //   0  SIMLOD_REGION_*; planes in use (PLANES only)
+    float    box_min[3], box_max[3];                //   8  BOX:    min <= p <= max on every axis
+    float    center[3], radius;                     //  32  SPHERE: |p - center|^2 <= radius^2
+    float    planes[SIMLOD_REGION_MAX_PLANES][4];   //  48  PLANES: n.p + d >= 0 for each of the first num_planes, (nx, ny, nz, d)
+} SimlodRegion;
+SIMLOD_STATIC_ASSERT(sizeof(SimlodRegion) == 304, "Region");
+SIMLOD_STATIC_ASSERT(offsetof(SimlodRegion, box_min) == 8 && offsetof(SimlodRegion, box_max) == 20, "Region.box");
+SIMLOD_STATIC_ASSERT(offsetof(SimlodRegion, center) == 32 && offsetof(SimlodRegion, radius) == 44, "Region.sphere");
+SIMLOD_STATIC_ASSERT(offsetof(SimlodRegion, planes) == 48, "Region.planes");
+enum { SIMLOD_CLIP_NONE = 0, SIMLOD_CLIP_INSIDE = 1, SIMLOD_CLIP_OUTSIDE = 2 };
+#define SIMLOD_CLIP_MAX_REGIONS 4
+typedef struct SimlodClip {
+    uint32_t     mode, num_regions;                         //   0  SIMLOD_CLIP_*; regions in use
+    SimlodRegion regions[SIMLOD_CLIP_MAX_REGIONS];          //   8  (304 bytes each)
+} SimlodClip;
+SIMLOD_STATIC_ASSERT(sizeof(SimlodClip) == 1224, "Clip");
+SIMLOD_STATIC_ASSERT(offsetof(SimlodClip, regions) == 8, "Clip.regions");

@@ -146,6 +146,16 @@ class SimlodRegion(C.Structure):
                 ("center", C.c_float * 3), ("radius", C.c_float), ("planes", (C.c_float * 4) * REGION_MAX_PLANES)]
 
 
+CLIP_NONE, CLIP_INSIDE, CLIP_OUTSIDE = 0, 1, 2
+CLIP_MAX_REGIONS = 4
+
+
+class SimlodClip(C.Structure):
+    """SimlodClip: render() and pick() draw only the samples inside (INSIDE) or outside (OUTSIDE) the union of the first
+    num_regions regions."""
+    _fields_ = [("mode", C.c_uint32), ("num_regions", C.c_uint32), ("regions", SimlodRegion * CLIP_MAX_REGIONS)]
+
+
 class SimlodQueryInfo(C.Structure):
     """SimlodQueryInfo: what a region query returned and how much of the octree it had to look at."""
     _fields_ = [("num_samples", C.c_uint64), ("num_points", C.c_uint64), ("num_voxels", C.c_uint64), ("samples_tested", C.c_uint64),
@@ -272,6 +282,7 @@ assert C.sizeof(ExportInfo) == 32 and EXPORT_NODE_DTYPE.itemsize == 64
 assert C.sizeof(LasHeader) == 128
 assert C.sizeof(OctreeFileHeader) == 128
 assert C.sizeof(SimlodRegion) == 304 and C.sizeof(SimlodQueryInfo) == 40
+assert C.sizeof(SimlodClip) == 1224 and SimlodClip.regions.offset == 8
 assert C.sizeof(SimlodPickInfo) == 40 and C.sizeof(SimlodNearestInfo) == 64 and C.sizeof(SimlodRayInfo) == 56
 assert C.sizeof(SimlodRadiusInfo) == 64
 assert C.sizeof(SimlodHeightmap) == 24 and C.sizeof(SimlodHeightmapInfo) == 56
@@ -290,7 +301,7 @@ EXPORTS = [
     "simlod_export_octree", "simlod_export_view", "simlod_read_las_header", "simlod_insert_files",
     "simlod_read_octree_header", "simlod_save_octree", "simlod_load_octree", "simlod_query_region",
     "simlod_pick", "simlod_query_nearest", "simlod_query_ray", "simlod_query_radius", "simlod_write_las", "simlod_files_box",
-    "simlod_query_heightmap",
+    "simlod_query_heightmap", "simlod_set_clip",
 ]
 
 _lib = None
@@ -354,6 +365,7 @@ def load_library():
         "simlod_save_octree": [vp, C.c_char_p, C.POINTER(ExportInfo), C.POINTER(C.c_float)],
         "simlod_load_octree": [vp, C.c_char_p, C.c_int, C.POINTER(ExportInfo), C.POINTER(C.c_float)],
         "simlod_query_region": [vp, C.POINTER(SimlodRegion), C.c_int32, u64, u64, C.POINTER(SimlodQueryInfo), C.POINTER(C.c_float)],
+        "simlod_set_clip": [vp, C.POINTER(SimlodClip)],
         "simlod_pick": [vp, C.POINTER(C.c_uint32), u64, u64, u64, C.POINTER(SimlodPickInfo), C.POINTER(C.c_float)],
         "simlod_query_nearest": [vp, u64, u64, u32, C.c_int32, C.c_float, u64, u64, u64, C.POINTER(SimlodNearestInfo),
                                  C.POINTER(C.c_float)],
@@ -803,6 +815,24 @@ class SimLOD:
                 if s.batchletIndex >= done:
                     break
         return total
+
+    def set_clip(self, regions, mode="inside"):
+        """Clip what render() and pick() draw (simlod_set_clip): with mode="inside" only the samples of the LOD cut inside
+        `regions`, with mode="outside" only those outside. `regions` is one Region (Region.box / sphere / planes) or a
+        list of up to 4, whose union is clipped by; a sample is inside by the region query's float32 predicate on its
+        stored x, y, z. None clears the clip. The cut, the visibility flags, stats() and export_view() do not change, so
+        pick indices stay indices into export_view().samples. The clip stays until it is set again. A malformed region,
+        an empty list or more than 4 regions raise SimlodError(-2) and leave the previous clip in place."""
+        clip = SimlodClip()
+        if regions is not None:
+            modes = {"inside": CLIP_INSIDE, "outside": CLIP_OUTSIDE}
+            if mode not in modes:
+                raise ValueError("mode must be 'inside' or 'outside', not %r" % (mode,))
+            regions = [regions] if isinstance(regions, SimlodRegion) else list(regions)
+            clip.mode, clip.num_regions = modes[mode], len(regions)
+            for k, r in enumerate(regions[:CLIP_MAX_REGIONS]):
+                clip.regions[k] = r
+        self._check(self._lib.simlod_set_clip(self._ctx, C.byref(clip)))
 
     def render(self):
         ms = C.c_float(0)

@@ -68,7 +68,8 @@ def build_native(force=False, verbose=False):
                os.path.join(CSRC, "fpmath.cuh"), os.path.join(CSRC, "lodcut.cuh"), os.path.join(CSRC, "loader_pool.h"),
                os.path.join(CSRC, "construct_layout.cuh"), os.path.join(CSRC, "export_common.cuh"), os.path.join(CSRC, "region.cuh"),
                os.path.join(CSRC, "search_common.cuh"),
-               os.path.join(CSRC, "kernel_args.h"), os.path.join(CSRC, "render_layout.cuh"), os.path.join(CSRC, "splat.cuh")]
+               os.path.join(CSRC, "kernel_args.h"), os.path.join(CSRC, "render_layout.cuh"), os.path.join(CSRC, "render_frame.inc"),
+               os.path.join(CSRC, "splat.cuh")]
     sources = [os.path.join(CSRC, name + ".cu") for name in PROGRAMS] + [os.path.join(CSRC, "host.cpp")]
     digest = _digest(sources + headers, " ".join(ARCH) + " -O3 -lineinfo " + repr(sorted(EXTRA_FLAGS.items())))
     stamp = os.path.join(CUBIN_DIR, "BUILD_STAMP")

@@ -57,8 +57,9 @@ struct PickArgs {                         // the view export's plan (export scra
     uint64_t* hits;                       // picked pixels among those the write kernel visits
     uint64_t numItems;
     uint32_t numRecords, pad;
+    SimlodClip clip;                      // the context's clip: candidates are the samples it keeps (mode NONE: all)
 };
-static_assert(sizeof(PickArgs) == 64 && offsetof(PickArgs, numItems) == 48, "PickArgs");
+static_assert(sizeof(PickArgs) == 1288 && offsetof(PickArgs, numItems) == 48 && offsetof(PickArgs, clip) == 64, "PickArgs");
 
 // ---- k nearest samples (nearest.cu) ----------------------------------------------------------------------------------
 

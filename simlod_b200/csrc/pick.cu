@@ -17,6 +17,7 @@
 #include "../../include/simlod_abi.h"
 #include "splat.cuh"
 #include "export_common.cuh"
+#include "region.cuh"
 
 constexpr uint64_t NO_INDEX = ~0ull;
 constexpr uint32_t PICK_UNROLL = 4;
@@ -41,7 +42,8 @@ simlod_pick_clear(const SimlodUniforms u, const PickArgs a) {
 // The key pass (indexPass false) and the index pass (true). The candidates, their keys and the pixels they cover are
 // kernel_render's (render.cu, all four draw paths): project(), inside (and depth > 0 with HQS), sampleColor() with the
 // record's level and node colour id, pixels clamp(x + ox, 0, W) + W clamp(y + oy, 0, H) for 0 <= ox, oy < pointSize.
-// Ids >= W*H lie outside the frame (the renderer's stores there land behind it) and are dropped.
+// Ids >= W*H lie outside the frame (the renderer's stores there land behind it) and are dropped. A sample the clip drops
+// (region.cuh clipKeeps, as simlod_render_clip tests it) is no candidate.
 template <bool indexPass>
 __device__ __forceinline__ void pickPass(const SimlodUniforms& u, const PickArgs& a) {
     if (!u.showPoints) return;
@@ -72,7 +74,7 @@ __device__ __forceinline__ void pickPass(const SimlodUniforms& u, const PickArgs
 #pragma unroll
             for (uint32_t s = 0; s < PICK_UNROLL; s++) {
                 const uint32_t j = b + s * 32 + lane;
-                if (j >= count) continue;
+                if (j >= count || !clipKeeps(a.clip, __uint_as_float(v[s].x), __uint_as_float(v[s].y), __uint_as_float(v[s].z))) continue;
                 const Projected pr = project(T, u.width, u.height, __uint_as_float(v[s].x), __uint_as_float(v[s].y), __uint_as_float(v[s].z));
                 if (!pr.inside || (hqs && !(pr.depth > 0.0f))) continue;
                 const uint64_t key = ((uint64_t)__float_as_uint(pr.depth) << 32) | sampleColor(u, v[s].w, level, colorId);

@@ -1,5 +1,5 @@
 // region.cuh — the two per-sample predicates of the region query (DESIGN.md §9.8), stated once for the count and the
-// write kernel of query.cu. Every operation is an explicit fpx:: instruction (round to nearest, no contraction), so the
+// write kernel of query.cu, and the clip test that render.cu and pick.cu build on the first of them (§9.15). Every operation is an explicit fpx:: instruction (round to nearest, no contraction), so the
 // numpy float32 restatement of the tests (tests/query_restatement.py) agrees in the last bit.
 #pragma once
 #include <stdint.h>
@@ -31,6 +31,16 @@ __device__ __forceinline__ bool regionContains(const SimlodRegion& r, float x, f
         in = in && v >= 0.0f;
     }
     return in;
+}
+
+// Clip predicate of render.cu and pick.cu (DESIGN.md §9.15): whether a sample at (x, y, z) is drawn under `c`. It is in
+// when regionContains holds for one of the first num_regions regions; INSIDE keeps what is in, OUTSIDE what is not, NONE
+// everything.
+__device__ __forceinline__ bool clipKeeps(const SimlodClip& c, float x, float y, float z) {
+    if (c.mode == SIMLOD_CLIP_NONE) return true;
+    bool in = false;
+    for (uint32_t k = 0; k < c.num_regions && !in; k++) in = regionContains(c.regions[k], x, y, z);
+    return c.mode == SIMLOD_CLIP_OUTSIDE ? !in : in;
 }
 
 // In-cube predicate: the point is not below boxMin and its 2^20 lattice coordinate (the builder's quantize(), construct.cu)
